@@ -656,8 +656,10 @@ int encode_stage(b200c_job* j, KeyCols mcols, uint64_t n_out, uint32_t min_s1, u
       j->kt_end(slot, j->st2);
     }
     CU(cudaEventRecord(j->evx[3], j->st2));
+    uint64_t data_bytes = 0;
+    for (uint32_t f = 0; f < nfiles; f++) data_bytes += frs[f].data_size;
     j->kt_begin("encode.emit");
-    launch_encode_emit(mcols, ep, W, nblocks, out_base_d, err, j->sms, st);
+    launch_encode_emit(mcols, ep, W, nblocks, out_base_d, data_bytes, err, j->sms, st);
     j->kt_end();
     launches += 3;
     if (P.bloom_millibits_per_key) {

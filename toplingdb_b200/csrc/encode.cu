@@ -1260,7 +1260,7 @@ __global__ void encode_filestats_kernel(KeyCols m, EncodeWork wk, uint32_t nfile
 }
 
 // ------------------------------------------------------------------------------------------------ emit data blocks
-constexpr int kEmitWarps = 8;
+constexpr int kEmitWarps = 4;
 // copy n bytes to generic dst from global src, one lane
 __device__ __forceinline__ void lane_copy(uint8_t* dst, const uint8_t* src, uint32_t n) {
   for (uint32_t i = 0; i < n; i++) dst[i] = src[i];
@@ -1562,14 +1562,326 @@ __device__ __forceinline__ void store_value_words(uint8_t* dst, const uint32_t* 
 }
 constexpr int kEmitPerLane = 3;
 constexpr int kEmitMaxEntries = 32 * kEmitPerLane;  // 96 entries per block on the fast path
+// ---- pieces both emit kernels share.  Lane-level: the header + key suffix of entry x (image offset off, pk = shared | ulen << 8 |
+// restart << 16) and its restart-array slot; returns the image offset of the entry's value bytes.
+__device__ __forceinline__ uint32_t emit_entry_key(uint8_t* img, uint32_t off, uint32_t pk, uint32_t vs, uint64_t hi, uint64_t lo, uint64_t tr,
+                                                   uint32_t x, uint32_t body, uint32_t R, uint32_t rmask) {
+  const uint32_t sh = pk & 0xff, ul = (pk >> 8) & 0xff;
+  uint8_t* p = img + off;
+  const uint32_t ks = ul + 8;
+  uint64_t S0, S1, S2;
+  key_suffix_words(hi, lo, ul, tr, sh, &S0, &S1, &S2);
+  if ((sh | (ks - sh) | vs) < 128) {
+    // three one-byte lengths + key suffix as one 27-byte stream
+    const uint64_t hdr = (uint64_t)sh | ((uint64_t)(ks - sh) << 8) | ((uint64_t)vs << 16);
+    const uint64_t W0 = hdr | (S0 << 24), W1 = (S0 >> 40) | (S1 << 24), W2 = (S1 >> 40) | (S2 << 24), W3 = S2 >> 40;
+    const uint32_t wv[8] = {(uint32_t)W0, (uint32_t)(W0 >> 32), (uint32_t)W1, (uint32_t)(W1 >> 32),
+                            (uint32_t)W2, (uint32_t)(W2 >> 32), (uint32_t)W3, 0u};
+    store_stream28(p, wv, 3 + ks - sh);
+    p += 3 + ks - sh;
+  } else {
+    p += put_varint(p, sh);
+    p += put_varint(p, ks - sh);
+    p += put_varint(p, vs);
+    store_bytes24(p, S0, S1, S2, ks - sh);
+    p += ks - sh;
+  }
+  if (pk >> 16) {  // restart array slot (block_builder.cc:207-210,128-133)
+    uint8_t* rp = img + body + 4u * (rmask != 0xffffffffu ? x >> __popc(rmask) : x / R);
+    rp[0] = (uint8_t)off;
+    rp[1] = (uint8_t)(off >> 8);
+    rp[2] = (uint8_t)(off >> 16);
+    rp[3] = (uint8_t)(off >> 24);
+  }
+  return (uint32_t)(p - img);
+}
+// Warp-level: one value of vl (> 64) bytes from sp to dp, aligned 4-byte source words funnel-shifted into byte stores.  Up to 512
+// bytes per pass: all of a pass's loads are issued before the first store, so a value of up to 512 bytes costs one memory round
+// trip, not one per 128 bytes.
+__device__ __forceinline__ void emit_copy_long_value(uint8_t* dp, const uint8_t* sp, uint32_t vl, unsigned lane) {
+  const uint32_t a = (uint32_t)((uintptr_t)sp & 3);
+  const uint32_t* wsrc = reinterpret_cast<const uint32_t*>((uintptr_t)sp - a);
+  const uint32_t nwords = (vl + 3) >> 2;
+  for (uint32_t k0 = 0; k0 < nwords; k0 += 128) {
+    uint32_t lo[4], hi[4];
+#pragma unroll
+    for (int t = 0; t < 4; t++) {
+      const uint32_t k = k0 + lane + 32 * t;
+      lo[t] = k < nwords ? __ldg(wsrc + k) : 0u;
+      hi[t] = k < nwords ? __ldg(wsrc + k + 1) : 0u;
+    }
+#pragma unroll
+    for (int t = 0; t < 4; t++) {
+      const uint32_t k = k0 + lane + 32 * t;
+      if (k < nwords) {
+        const uint32_t v = __funnelshift_r(lo[t], hi[t], a * 8);
+        const uint32_t o = 4 * k;
+        dp[o] = (uint8_t)v;
+        if (o + 1 < vl) dp[o + 1] = (uint8_t)(v >> 8);
+        if (o + 2 < vl) dp[o + 2] = (uint8_t)(v >> 16);
+        if (o + 3 < vl) dp[o + 3] = (uint8_t)(v >> 24);
+      }
+    }
+  }
+}
+// Warp-level: restart count footer, checksum trailer, then the image (built at gdst's 16-byte phase `shift`) leaves as head bytes,
+// ONE bulk copy (TMA) of everything between the first and the last 16-byte boundary, and tail bytes
+__device__ __forceinline__ void emit_block_finish(uint8_t* img, uint8_t* gdst, uint32_t shift, uint32_t body, uint32_t nrest, uint32_t cksum,
+                                                  uint32_t xtab, unsigned lane) {
+  const uint32_t payload = body + 4 * nrest + 4;
+  if (lane == 0) {
+    uint8_t* fp = img + body + 4u * nrest;
+    fp[0] = (uint8_t)nrest;
+    fp[1] = (uint8_t)(nrest >> 8);
+    fp[2] = (uint8_t)(nrest >> 16);
+    fp[3] = (uint8_t)(nrest >> 24);
+  }
+  __syncwarp();
+  const uint32_t ck = staged_block_checksum(cksum, (uint32_t)__cvta_generic_to_shared(img), img, payload, 0, xtab, lane);
+  __syncwarp();  // the checksum's 8-byte loads may touch the trailer bytes written next
+  if (lane == 0) {
+    uint8_t* tp = img + payload;
+    tp[0] = 0;
+    tp[1] = (uint8_t)ck;
+    tp[2] = (uint8_t)(ck >> 8);
+    tp[3] = (uint8_t)(ck >> 16);
+    tp[4] = (uint8_t)(ck >> 24);
+  }
+  fence_async_smem();  // this lane's image bytes are visible to the TMA engine
+  __syncwarp();
+  const uint32_t total = payload + 5;
+  uint32_t head = shift ? 16 - shift : 0;
+  if (head > total) head = total;
+  const uint32_t mid = (total - head) & ~15u;
+  if (lane == 0 && mid) bulk_s2g(gdst + head, (uint32_t)__cvta_generic_to_shared(img + head), mid);
+  if (lane < head) gdst[lane] = img[lane];
+  const uint32_t done = head + mid;
+  if (done + lane < total) gdst[done + lane] = img[done + lane];
+}
+constexpr int kEmitCtasPerSm = 3;                   // 12 warps per SM (with kEmitWarps = 4): room for 168 registers, no spills
+// A column stage holds one block's entries of every column, copied by TMA as the 16-byte-aligned cover of the entry range (the cover
+// starts up to 15 bytes before the range and ends up to 15 bytes behind it, so a region holds kEmitMaxEntries elements + 16 bytes).
+// Every 16-byte unit the cover reads holds at least one byte of the column, so it lies in a page the column occupies; the bytes
+// around the range are never used.  On the compaction path the columns are DevBuf allocations with >= 256 bytes of slack, so the
+// cover stays inside them; columns a caller hands to b200c_job_encode_columns may end within 15 bytes of the cover's end, and
+// those reads then pass the end of the caller's allocation (but not of its page).  The 16-byte value loads below rely on the same
+// property: a chunk is read only when it holds a byte of the value.
+constexpr uint32_t kStPfx = 0, kStTr = kStPfx + 16 * kEmitMaxEntries + 16, kStVref = kStTr + 8 * kEmitMaxEntries + 16,
+                   kStMeta = kStVref + 8 * kEmitMaxEntries + 16, kStEsh = kStMeta + 4 * kEmitMaxEntries + 16,
+                   kStageBytes = kStEsh + kEmitMaxEntries + 16;
+static_assert(kStTr % 16 == 0 && kStVref % 16 == 0 && kStMeta % 16 == 0 && kStEsh % 16 == 0 && kStageBytes % 16 == 0,
+              "bulk copies need 16-byte aligned shared-memory destinations");
+__device__ __forceinline__ uint32_t cover16(const void* p, uint32_t bytes, uintptr_t* a0) {
+  *a0 = (uintptr_t)p & ~(uintptr_t)15;
+  return (uint32_t)((((uintptr_t)p + bytes + 15) & ~(uintptr_t)15) - *a0);
+}
+// lane 0: start the bulk copies of the columns of entries [e0, e0 + E) into the stage at shared address `stage`, completing on `bar`
+__device__ __forceinline__ void emit_stage_fill(const KeyCols& m, const EncodeWork& wk, uint64_t e0, uint32_t E, uint32_t stage, uint32_t bar) {
+  uintptr_t a[5];
+  const uint32_t n0 = cover16(m.pfx + e0, 16 * E, &a[0]), n1 = cover16(m.tr + e0, 8 * E, &a[1]), n2 = cover16(m.vref + e0, 8 * E, &a[2]),
+                 n3 = cover16(m.meta + e0, 4 * E, &a[3]), n4 = cover16(wk.eshared + e0, E, &a[4]);
+  mbar_expect_tx(bar, n0 + n1 + n2 + n3 + n4);
+  bulk_g2s(stage + kStPfx, reinterpret_cast<const void*>(a[0]), n0, bar);
+  bulk_g2s(stage + kStTr, reinterpret_cast<const void*>(a[1]), n1, bar);
+  bulk_g2s(stage + kStVref, reinterpret_cast<const void*>(a[2]), n2, bar);
+  bulk_g2s(stage + kStMeta, reinterpret_cast<const void*>(a[3]), n3, bar);
+  bulk_g2s(stage + kStEsh, reinterpret_cast<const void*>(a[4]), n4, bar);
+}
 // One WARP per data block, no CTA-wide synchronisation: lane l owns the block's entries [3l, 3l + 3), a warp scan of the
+// entry sizes gives every entry its byte position, the lanes write header + key suffix + value into the warp's block
+// image in shared memory, then the warp appends restart array + footer, checksums the image and stores it re-aligned
+// to the file offset.  The block's columns arrive in shared memory ahead of time: while the warp builds one block, lane 0 has
+// TMA copy the next block's columns into the other of the warp's two stages.  The only DRAM round trip a block still waits
+// for is its value words, and the key bytes are written while those loads are in flight.  Blocks with more than 96 entries
+// or larger than the image slot take emit_block_warp (no stage: it reads the columns from global memory).
+__global__ void __launch_bounds__(kEmitWarps * 32, kEmitCtasPerSm)
+encode_emit_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t nblocks, uint8_t* const* __restrict__ out_base,
+                   uint32_t slot_bytes, uint32_t* __restrict__ err) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  __shared__ XxhLaneTab s_xtab;
+  __shared__ __align__(8) uint64_t s_bar[kEmitWarps][2];
+  const unsigned lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  uint8_t* const slot = smem + (size_t)w * slot_bytes;  // 16-byte aligned (slot_bytes is a multiple of 256)
+  uint8_t* const stages = smem + (size_t)kEmitWarps * slot_bytes + (size_t)w * 2 * kStageBytes;
+  const uint32_t stages_sa = (uint32_t)__cvta_generic_to_shared(stages), bar0 = (uint32_t)__cvta_generic_to_shared(&s_bar[w][0]);
+  fill_xxh_lane_tab(&s_xtab);
+  if (lane == 0) {
+    mbar_init(bar0, 1);
+    mbar_init(bar0 + 8, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  const uint32_t xtab = (uint32_t)__cvta_generic_to_shared(&s_xtab);
+  const uint32_t R = ep.restart_interval;
+  const uint32_t rmask = (R & (R - 1)) == 0 ? R - 1 : 0xffffffffu;  // power-of-two restart interval: mask instead of %
+  const uint64_t stride = (uint64_t)gridDim.x * kEmitWarps;
+  uint64_t b = (uint64_t)blockIdx.x * kEmitWarps + w;
+  // br = this block, brn = the warp's next block: its stage fill is issued at the top of the iteration.  The records of the two
+  // blocks after this one are (re)loaded into nbr / nbrn before the checksum, which hides their latency and keeps them out of
+  // the registers the entry work needs.
+  BlockRec br{}, brn{}, nbr{}, nbrn{};
+  if (b < nblocks) br = wk.blocks[b];
+  if (b + stride < nblocks) brn = wk.blocks[b + stride];
+  if (lane == 0 && b < nblocks && br.n_entries <= (uint32_t)kEmitMaxEntries) emit_stage_fill(m, wk, br.first_entry, br.n_entries, stages_sa, bar0);
+  uint32_t s = 0, parity = 0;  // stage of block b; bit t of parity = phase parity of stage t's next completion
+  for (; b < nblocks; b += stride, s ^= 1, br = nbr, brn = nbrn) {
+    __syncwarp();
+    if (lane == 0 && b + stride < nblocks && brn.n_entries <= (uint32_t)kEmitMaxEntries) {
+      // every lane finished reading stage s ^ 1 (the previous block; __syncwarp above): order those generic-proxy reads before
+      // the async-proxy writes of the refill
+      fence_async_smem();
+      emit_stage_fill(m, wk, brn.first_entry, brn.n_entries, stages_sa + (s ^ 1) * kStageBytes, bar0 + 8 * (s ^ 1));
+    }
+    auto load_next = [&]() {
+      if (b + stride < nblocks) nbr = wk.blocks[b + stride];
+      if (b + 2 * stride < nblocks) nbrn = wk.blocks[b + 2 * stride];
+    };
+    const uint32_t E = br.n_entries;
+    const uint64_t e0 = br.first_entry;
+    // The image is built at the destination's 16-byte phase, so that everything between the first and the last 16-byte boundary
+    // of the block leaves shared memory as ONE bulk copy (TMA) instead of a load / re-align / store loop.
+    uint8_t* const gdst = out_base[br.file_idx] + br.file_off;
+    const uint32_t shift = (uint32_t)((uintptr_t)gdst & 15);
+    uint8_t* const img = slot + shift;
+    if (E > (uint32_t)kEmitMaxEntries) {
+      load_next();
+      if (lane == 0) bulk_wait_read0();  // the previous block's bulk store has finished reading the slot
+      __syncwarp();
+      emit_block_warp(m, ep, wk, b, out_base, slot, slot_bytes);
+      continue;
+    }
+    // the block's columns in stage s, each at the 16-byte phase of its global address
+    const uint8_t* const stg = stages + s * kStageBytes;
+    const ulonglong2* const c_pfx = reinterpret_cast<const ulonglong2*>(stg + kStPfx + ((uintptr_t)(m.pfx + e0) & 15));
+    const uint64_t* const c_tr = reinterpret_cast<const uint64_t*>(stg + kStTr + ((uintptr_t)(m.tr + e0) & 15));
+    const uint64_t* const c_vref = reinterpret_cast<const uint64_t*>(stg + kStVref + ((uintptr_t)(m.vref + e0) & 15));
+    const uint32_t* const c_meta = reinterpret_cast<const uint32_t*>(stg + kStMeta + ((uintptr_t)(m.meta + e0) & 15));
+    const uint8_t* const c_esh = stg + kStEsh + ((uintptr_t)(wk.eshared + e0) & 15);
+    mbar_wait(bar0 + 8 * s, (parity >> s) & 1);
+    parity ^= 1u << s;
+    // ---- sizes
+    uint32_t sz[kEmitPerLane], pk[kEmitPerLane], vs[kEmitPerLane];  // pk = shared | ulen << 8 | restart << 16
+    uint32_t tsum = 0;
+#pragma unroll
+    for (int i = 0; i < kEmitPerLane; i++) {
+      const uint32_t x = lane * kEmitPerLane + i;
+      sz[i] = pk[i] = vs[i] = 0;
+      if (x < E) {
+        const uint32_t mt = c_meta[x];
+        const bool restart = (rmask != 0xffffffffu ? (x & rmask) : (x % R)) == 0;
+        const uint32_t ul = meta_ulen(mt);
+        vs[i] = meta_vlen(mt);
+        const uint32_t sh = restart ? 0 : c_esh[x];
+        pk[i] = sh | (ul << 8) | (restart ? 1u << 16 : 0);
+        sz[i] = entry_size(sh, ul + 8, vs[i]);
+        tsum += sz[i];
+      }
+    }
+    const uint64_t inc = warp_incl_scan64(tsum);
+    const uint64_t body64 = __shfl_sync(0xffffffffu, inc, 31);
+    const uint32_t nrest = (E + R - 1) / R;
+    if (body64 + 4ull * nrest + 4 + 5 + 32 + 16 > slot_bytes) {  // uniform
+      load_next();
+      if (lane == 0) bulk_wait_read0();
+      __syncwarp();
+      emit_block_warp(m, ep, wk, b, out_base, slot, slot_bytes);
+      continue;
+    }
+    const uint32_t body = (uint32_t)body64;
+    uint32_t off[kEmitPerLane];
+    {
+      uint32_t run = (uint32_t)(inc - tsum);
+#pragma unroll
+      for (int i = 0; i < kEmitPerLane; i++) {
+        off[i] = run;
+        run += sz[i];
+      }
+    }
+    // ---- value bytes of all the lane's entries (when every value is short) leave first; the key bytes are written meanwhile.
+    // A value of <= 32 bytes lies in at most three aligned 16-byte chunks: three vector loads instead of nine word loads (the
+    // lanes' values are scattered, so every load instruction touches one cache line per lane).  Value references are read from
+    // the stage where they are used, so that no register holds them across the key work.
+    constexpr int kNW = 9;  // aligned words covering a value of <= 32 bytes at any 4-byte phase
+    bool all_short = true;
+#pragma unroll
+    for (int i = 0; i < kEmitPerLane; i++) all_short = all_short && vs[i] <= 32;
+    uint4 vc[kEmitPerLane][3];
+    if (all_short) {
+#pragma unroll
+      for (int i = 0; i < kEmitPerLane; i++) {
+        const uint64_t vr = vs[i] ? c_vref[lane * kEmitPerLane + i] : 0;  // (vs[i] == 0 beyond the block's entries)
+        const uint32_t a = (uint32_t)(vr & 15);
+        const uint4* csrc = reinterpret_cast<const uint4*>((uintptr_t)vr - a);
+        const uint32_t nc = vs[i] ? (a + vs[i] + 15) >> 4 : 0;
+#pragma unroll
+        for (int k = 0; k < 3; k++) vc[i][k] = (uint32_t)k < nc ? __ldg(csrc + k) : make_uint4(0, 0, 0, 0);
+      }
+    }
+    if (lane == 0) bulk_wait_read0();  // the previous block's bulk store has finished reading the slot
+    __syncwarp();
+    uint32_t voff[kEmitPerLane];  // image offset of the value bytes
+#pragma unroll
+    for (int i = 0; i < kEmitPerLane; i++) {
+      const uint32_t x = lane * kEmitPerLane + i;
+      voff[i] = 0;
+      if (x < E) {
+        const ulonglong2 pp = c_pfx[x];
+        voff[i] = emit_entry_key(img, off[i], pk[i], vs[i], pp.x, pp.y, c_tr[x], x, body, R, rmask);
+      }
+    }
+    if (all_short) {
+#pragma unroll
+      for (int i = 0; i < kEmitPerLane; i++) {
+        if (!vs[i]) continue;
+        const uint32_t a = (uint32_t)(c_vref[lane * kEmitPerLane + i] & 15);
+        uint32_t w[12] = {vc[i][0].x, vc[i][0].y, vc[i][0].z, vc[i][0].w, vc[i][1].x, vc[i][1].y,
+                          vc[i][1].z, vc[i][1].w, vc[i][2].x, vc[i][2].y, vc[i][2].z, vc[i][2].w};
+        // drop the a / 4 words in front of the value: w[0..kNW) then covers it at the 4-byte phase a & 3 (a & 3 + 32 bytes end
+        // inside w[8]), and w[kNW] = 0 as store_value_words expects
+        if (a & 8) {
+#pragma unroll
+          for (int k = 0; k < 10; k++) w[k] = w[k + 2];
+        }
+        if (a & 4) {
+#pragma unroll
+          for (int k = 0; k < 11; k++) w[k] = w[k + 1];
+        }
+        w[kNW] = 0;
+        store_value_words<kNW>(img + voff[i], w, a & 3, vs[i]);
+      }
+    } else {
+#pragma unroll
+      for (int i = 0; i < kEmitPerLane; i++)
+        if (vs[i] && vs[i] <= 64) copy_value_small(img + voff[i], (const uint8_t*)(uintptr_t)c_vref[lane * kEmitPerLane + i], vs[i]);
+    }
+    // values longer than 64 bytes: the warp copies each of them with all lanes
+#pragma unroll
+    for (int i = 0; i < kEmitPerLane; i++) {
+      unsigned big = __ballot_sync(0xffffffffu, vs[i] > 64);
+      while (big) {
+        const int sl = __ffs(big) - 1;
+        big &= big - 1;
+        const uint32_t vl = __shfl_sync(0xffffffffu, vs[i], sl);
+        const uint32_t vo = __shfl_sync(0xffffffffu, voff[i], sl);
+        emit_copy_long_value(img + vo, (const uint8_t*)(uintptr_t)c_vref[sl * kEmitPerLane + i], vl, lane);
+      }
+    }
+    load_next();
+    emit_block_finish(img, gdst, shift, body, nrest, ep.checksum, xtab, lane);
+  }
+  if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // no bulk store may outlive the CTA's shared memory
+  (void)err;
+}
+
+constexpr int kEmitLongWarps = 8, kEmitLongCtasPerSm = 4;  // 32 warps per SM, 64 registers each
+// Jobs whose entries are all long (the value path below copies them warp-wide): more warps per SM with fewer registers each,
+// and no column stages.  One WARP per data block, no CTA-wide synchronisation: lane l owns the block's entries [3l, 3l + 3), a warp scan of the
 // entry sizes gives every entry its byte position, the lanes write header + key suffix + value into the warp's block
 // image in shared memory, then the warp appends restart array + footer, checksums the image and stores it re-aligned
 // to the file offset.  Global loads are issued in groups (size columns; key columns; value words) so that a block costs
 // three DRAM round trips.  Blocks with more than 96 entries or larger than the image slot take emit_block_warp.
-template <int kMinCtas>
-__global__ void __launch_bounds__(kEmitWarps * 32, kMinCtas)
-encode_emit_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t nblocks, uint8_t* const* __restrict__ out_base,
+__global__ void __launch_bounds__(kEmitLongWarps * 32, kEmitLongCtasPerSm)
+encode_emit_long_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t nblocks, uint8_t* const* __restrict__ out_base,
                    uint32_t slot_bytes, uint32_t* __restrict__ err) {
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ XxhLaneTab s_xtab;
@@ -1580,8 +1892,8 @@ encode_emit_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t nblocks, 
   const uint32_t xtab = (uint32_t)__cvta_generic_to_shared(&s_xtab);
   const uint32_t R = ep.restart_interval;
   const uint32_t rmask = (R & (R - 1)) == 0 ? R - 1 : 0xffffffffu;  // power-of-two restart interval: mask instead of %
-  const uint64_t stride = (uint64_t)gridDim.x * kEmitWarps;
-  for (uint64_t b = (uint64_t)blockIdx.x * kEmitWarps + w; b < nblocks; b += stride) {
+  const uint64_t stride = (uint64_t)gridDim.x * kEmitLongWarps;
+  for (uint64_t b = (uint64_t)blockIdx.x * kEmitLongWarps + w; b < nblocks; b += stride) {
     const BlockRec br = wk.blocks[b];
     const uint32_t E = br.n_entries;
     const uint64_t e0 = br.first_entry;
@@ -1670,34 +1982,7 @@ encode_emit_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t nblocks, 
         const uint32_t x = lane * kEmitPerLane + i;
         voff[i] = 0;
         if (x < E) {
-          const uint32_t sh = pk[i] & 0xff, ul = (pk[i] >> 8) & 0xff;
-          uint8_t* p = img + off[i];
-          const uint32_t ks = ul + 8;
-          uint64_t S0, S1, S2;
-          key_suffix_words(ppv[i].x, ppv[i].y, ul, trv[i], sh, &S0, &S1, &S2);
-          if ((sh | (ks - sh) | vs[i]) < 128) {
-            // three one-byte lengths + key suffix as one 27-byte stream
-            const uint64_t hdr = (uint64_t)sh | ((uint64_t)(ks - sh) << 8) | ((uint64_t)vs[i] << 16);
-            const uint64_t W0 = hdr | (S0 << 24), W1 = (S0 >> 40) | (S1 << 24), W2 = (S1 >> 40) | (S2 << 24), W3 = S2 >> 40;
-            const uint32_t wv[8] = {(uint32_t)W0, (uint32_t)(W0 >> 32), (uint32_t)W1, (uint32_t)(W1 >> 32),
-                                    (uint32_t)W2, (uint32_t)(W2 >> 32), (uint32_t)W3, 0u};
-            store_stream28(p, wv, 3 + ks - sh);
-            p += 3 + ks - sh;
-          } else {
-            p += put_varint(p, sh);
-            p += put_varint(p, ks - sh);
-            p += put_varint(p, vs[i]);
-            store_bytes24(p, S0, S1, S2, ks - sh);
-            p += ks - sh;
-          }
-          voff[i] = (uint32_t)(p - img);
-          if (pk[i] >> 16) {
-            uint8_t* rp = img + body + 4u * (rmask != 0xffffffffu ? x >> __popc(rmask) : x / R);
-            rp[0] = (uint8_t)off[i];
-            rp[1] = (uint8_t)(off[i] >> 8);
-            rp[2] = (uint8_t)(off[i] >> 16);
-            rp[3] = (uint8_t)(off[i] >> 24);
-          }
+          voff[i] = emit_entry_key(img, off[i], pk[i], vs[i], ppv[i].x, ppv[i].y, trv[i], x, body, R, rmask);
         }
       }
     }
@@ -1735,52 +2020,10 @@ encode_emit_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t nblocks, 
         const uint32_t vl = __shfl_sync(0xffffffffu, vs[i], sl);
         const uint32_t vo = __shfl_sync(0xffffffffu, voff[i], sl);
         const uint64_t vrr = __shfl_sync(0xffffffffu, vrf[i], sl);
-        const uint8_t* sp = (const uint8_t*)(uintptr_t)vrr;
-        uint8_t* dp = img + vo;
-        // aligned 4-byte source words, funnel-shifted; byte stores into the image
-        const uint32_t a = (uint32_t)((uintptr_t)sp & 3);
-        const uint32_t* wsrc = reinterpret_cast<const uint32_t*>((uintptr_t)sp - a);
-        const uint32_t nwords = (vl + 3) >> 2;
-        for (uint32_t k = lane; k < nwords; k += 32) {
-          const uint32_t v = __funnelshift_r(__ldg(wsrc + k), __ldg(wsrc + k + 1), a * 8);
-          const uint32_t o = 4 * k;
-          dp[o] = (uint8_t)v;
-          if (o + 1 < vl) dp[o + 1] = (uint8_t)(v >> 8);
-          if (o + 2 < vl) dp[o + 2] = (uint8_t)(v >> 16);
-          if (o + 3 < vl) dp[o + 3] = (uint8_t)(v >> 24);
-        }
+        emit_copy_long_value(img + vo, (const uint8_t*)(uintptr_t)vrr, vl, lane);
       }
     }
-    // ---- restart footer, checksum trailer, store
-    const uint32_t payload = body + 4 * nrest + 4;
-    if (lane == 0) {
-      uint8_t* fp = img + body + 4u * nrest;
-      fp[0] = (uint8_t)nrest;
-      fp[1] = (uint8_t)(nrest >> 8);
-      fp[2] = (uint8_t)(nrest >> 16);
-      fp[3] = (uint8_t)(nrest >> 24);
-    }
-    __syncwarp();
-    const uint32_t ck = staged_block_checksum(ep.checksum, (uint32_t)__cvta_generic_to_shared(img), img, payload, 0, xtab, lane);
-    __syncwarp();  // the checksum's 8-byte loads may touch the trailer bytes written next
-    if (lane == 0) {
-      uint8_t* tp = img + payload;
-      tp[0] = 0;
-      tp[1] = (uint8_t)ck;
-      tp[2] = (uint8_t)(ck >> 8);
-      tp[3] = (uint8_t)(ck >> 16);
-      tp[4] = (uint8_t)(ck >> 24);
-    }
-    fence_async_smem();  // this lane's image bytes are visible to the TMA engine
-    __syncwarp();
-    const uint32_t total = payload + 5;
-    uint32_t head = shift ? 16 - shift : 0;
-    if (head > total) head = total;
-    const uint32_t mid = (total - head) & ~15u;
-    if (lane == 0 && mid) bulk_s2g(gdst + head, (uint32_t)__cvta_generic_to_shared(img + head), mid);
-    if (lane < head) gdst[lane] = img[lane];
-    const uint32_t done = head + mid;
-    if (done + lane < total) gdst[done + lane] = img[done + lane];
+    emit_block_finish(img, gdst, shift, body, nrest, ep.checksum, xtab, lane);
   }
   if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // no bulk store may outlive the CTA's shared memory
   (void)err;
@@ -2321,6 +2564,7 @@ void launch_encode_filestats(KeyCols m, EncodeWork w, uint32_t nfiles, int sms, 
   (void)sms;
   encode_filestats_kernel<<<nfiles, 256, 0, st>>>(m, w, nfiles);
 }
+constexpr uint32_t kEmitMaxSmem = 224 * 1024;  // dynamic shared memory of one emit CTA at most (+ ~2 KB static: XXH3 lane table, mbarriers)
 uint32_t encode_emit_slice(uint32_t block_size) {
   uint32_t s = block_size + block_size / 4 + 512;
   s = (s + 255) & ~255u;
@@ -2328,39 +2572,38 @@ uint32_t encode_emit_slice(uint32_t block_size) {
   if (s > 24 * 1024) s = 24 * 1024;
   return s;
 }
-void launch_encode_emit(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nblocks, uint8_t* const* out_base, uint32_t* err, int sms,
-                        cudaStream_t st) {
+static_assert(kEmitWarps * (24 * 1024 + 2 * kStageBytes) <= kEmitMaxSmem, "the largest slots and their column stages fit one CTA");
+void launch_encode_emit(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nblocks, uint8_t* const* out_base, uint64_t data_bytes,
+                        uint32_t* err, int sms, cudaStream_t st) {
   if (nblocks == 0) return;
-  static int occ = 0;
-  if (!occ) {
-    const char* e = getenv("B200C_EMIT_CTAS_PER_SM");  // tuning knob
-    occ = e && atoi(e) >= 3 && atoi(e) <= 5 ? atoi(e) : 4;  // 4: 64 registers with a small spill, but 32 independent warps per SM
-  }
   static PerDeviceFlag attr;
   const uint64_t dev_bit = attr.bit_of_current_device();
   if (!attr.is_set(dev_bit)) {
-    // (the kernel also has ~2 KB of static shared memory: the XXH3 lane table)
-    cudaFuncSetAttribute(encode_emit_kernel<5>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
-    cudaFuncSetAttribute(encode_emit_kernel<3>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
-    cudaFuncSetAttribute(encode_emit_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024);
+    cudaFuncSetAttribute(encode_emit_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kEmitMaxSmem);
+    cudaFuncSetAttribute(encode_emit_long_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kEmitMaxSmem);
     attr.set(dev_bit);
   }
+  // Mean on-disk bytes per entry above 64 (data_bytes: the job's data blocks with their trailers): most values are longer than the
+  // staged kernel's 32-byte vector path and go through per-lane word copies or the warp-wide copy, a chain of dependent loads per
+  // value.  The 32 warps per SM of the long-entry kernel hide those chains better than the staged kernel's 12 (measured on H100
+  // with 128 B and 256 B values: profiles/README.md).  A mean, unlike the smallest entry, does not flip on a few tombstones or
+  // short values in a long-value job.
+  const bool long_entries = data_bytes > 64 * m.n;
+  const int warps = long_entries ? kEmitLongWarps : kEmitWarps, ctas = long_entries ? kEmitLongCtasPerSm : kEmitCtasPerSm;
   const uint32_t slot = encode_emit_slice(ep.block_size);
-  const size_t smem = (size_t)slot * kEmitWarps;
-  unsigned per_sm = (unsigned)((228 * 1024) / (smem + 1024 + 2048));
+  const size_t smem = (size_t)warps * (slot + (long_entries ? 0 : 2 * kStageBytes));
+  int per_sm = 0;  // resident CTAs per SM at this slot size (registers, static + dynamic shared memory)
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, long_entries ? (const void*)encode_emit_long_kernel : (const void*)encode_emit_kernel,
+                                                warps * 32, smem);
   if (per_sm < 1) per_sm = 1;
-  if (per_sm > (unsigned)occ) per_sm = (unsigned)occ;
-  const uint64_t want = (nblocks + kEmitWarps - 1) / kEmitWarps;
+  if (per_sm > ctas) per_sm = ctas;
+  const uint64_t want = (nblocks + warps - 1) / warps;
   // The persistent CTAs own every register of the SMs they sit on, so the side stream's kernels (per-file statistics, index
-  // blocks) queue behind the last emit CTA.  Leaving CTA slots free for them (B200C_EMIT_RESERVE = n slots) was
-  // measured and does not pay: 8 slots slowed the emit kernel down, 16 / 32 slots changed nothing.
-  static const int reserve = getenv("B200C_EMIT_RESERVE") ? atoi(getenv("B200C_EMIT_RESERVE")) : 0;
-  uint64_t cap = (uint64_t)sms * per_sm;
-  if (reserve > 0 && cap > 4 * (uint64_t)reserve) cap -= (uint64_t)reserve;
+  // blocks) queue behind the last emit CTA.
+  const uint64_t cap = (uint64_t)sms * per_sm;
   const unsigned grid = (unsigned)(want < cap ? want : cap);
-  if (occ == 4) encode_emit_kernel<4><<<grid, kEmitWarps * 32, smem, st>>>(m, ep, w, nblocks, out_base, slot, err);
-  else if (occ == 5) encode_emit_kernel<5><<<grid, kEmitWarps * 32, smem, st>>>(m, ep, w, nblocks, out_base, slot, err);
-  else encode_emit_kernel<3><<<grid, kEmitWarps * 32, smem, st>>>(m, ep, w, nblocks, out_base, slot, err);
+  if (long_entries) encode_emit_long_kernel<<<grid, warps * 32, smem, st>>>(m, ep, w, nblocks, out_base, slot, err);
+  else encode_emit_kernel<<<grid, warps * 32, smem, st>>>(m, ep, w, nblocks, out_base, slot, err);
 }
 void launch_encode_index(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nblocks, uint32_t nfiles, uint8_t* const* out_base,
                          uint32_t* err, int sms, cudaStream_t st, uint64_t* launches) {

@@ -242,9 +242,9 @@ void launch_encode_blocklist(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t 
                              cudaStream_t st);
 void launch_encode_filestats(KeyCols m, EncodeWork w, uint32_t nfiles, int sms, cudaStream_t st);
 uint32_t encode_emit_slice(uint32_t block_size);
-// out_base[f] = device address where file f's image starts; slice = shared-memory bytes per warp
-void launch_encode_emit(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nblocks, uint8_t* const* out_base, uint32_t* err,
-                        int sms, cudaStream_t st);
+// out_base[f] = device address where file f's image starts; data_bytes = all data blocks incl. trailers (with m.n: selects the kernel)
+void launch_encode_emit(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nblocks, uint8_t* const* out_base, uint64_t data_bytes,
+                        uint32_t* err, int sms, cudaStream_t st);
 void launch_encode_index(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nblocks, uint32_t nfiles, uint8_t* const* out_base,
                          uint32_t* err, int sms, cudaStream_t st, uint64_t* launches);
 void launch_block_checksums(uint32_t type, const uint8_t* data, const uint64_t* offsets, uint32_t n, uint8_t last_byte,
