@@ -246,7 +246,6 @@ struct b200c_job {
   DevBuf esz, eshared, tstat, nxt, disk, rows, tstate, grows, gstate, gflag, gsync, idx_contrib, idx_contrib_off, blocks, files_rec, idx_esz, idx_eoff, idx_sep, out_buf, out_base_d;
   uint64_t n_total = 0, n_out = 0, nblk_in = 0, nblocks_out = 0;
   uint32_t nfiles_out = 0, nruns = 0;
-  DevBuf tprefix2;  // stat-tile prefixes of the sizes pass (B200C_MERGE_FOLD=0)
   DevBuf bloom_contrib, bloom_contrib_off;  // scratch of the filter blocks' checksums
   DevBuf bloom_hashes;                      // key hashes of the output entries (filter policy jobs)
   DevBuf kv_arena, kv_offs, kv_klens;  // b200c_job_encode_kv: the caller's records on the device
@@ -596,11 +595,6 @@ int encode_stage(b200c_job* j, KeyCols mcols, uint64_t n_out, uint32_t min_s1, u
     }
     nblocks = h[kSlotTotals];
     nfiles = (uint32_t)h[kSlotTotals + 1];
-#ifdef B200C_STITCH_TRACE
-    fprintf(stderr, "stitch trace (cycles): walk %llu wait %llu refill_groups %llu (%llu) refill_tiles %llu (%llu) chase %llu (%llu); hc %u\n",
-            (unsigned long long)h[20], (unsigned long long)h[21], (unsigned long long)h[22], (unsigned long long)h[25], (unsigned long long)h[23],
-            (unsigned long long)h[26], (unsigned long long)h[24], (unsigned long long)h[27], hc);
-#endif
     if (nfiles == 0 || nfiles > kMaxOutFiles) return fail(B200C_ERR_CUDA, "internal: bad output file count");
     CU(j->blocks.reserve(sizeof(BlockRec) * (nblocks + 1)));
     CU(j->idx_esz.reserve(4 * (nblocks + 1)));
@@ -619,14 +613,6 @@ int encode_stage(b200c_job* j, KeyCols mcols, uint64_t n_out, uint32_t min_s1, u
       off += (cap + 255) & ~255ull;
     }
     base_off[nfiles] = off;
-    if (getenv("B200C_DEBUG_LAYOUT") || off > (1ull << 44)) {
-      fprintf(stderr, "[b200c] layout: n_out=%llu nblocks=%llu nfiles=%u off=%llu hc=%u etiles=%llu\n", (unsigned long long)n_out,
-              (unsigned long long)nblocks, nfiles, (unsigned long long)off, hc, (unsigned long long)etiles);
-      for (uint32_t f = 0; f < nfiles && f < 4; f++)
-        fprintf(stderr, "[b200c]  file %u: first_entry=%llu n_entries=%llu first_block=%llu n_blocks=%llu data_size=%llu filter_bytes=%llu\n", f,
-                (unsigned long long)frs[f].first_entry, (unsigned long long)frs[f].n_entries, (unsigned long long)frs[f].first_block,
-                (unsigned long long)frs[f].n_blocks, (unsigned long long)frs[f].data_size, (unsigned long long)frs[f].filter_bytes);
-    }
     CU(j->out_buf.reserve(off + 256));
     {  // scratch for the parallel part of the index-block checksum
       std::vector<uint64_t> coff(nfiles + 1, 0);
@@ -651,8 +637,8 @@ int encode_stage(b200c_job* j, KeyCols mcols, uint64_t n_out, uint32_t min_s1, u
     CU(cudaStreamWaitEvent(j->st2, j->evx[2], 0));
     {
       const size_t slot = j->kt_begin("~encode.filestats+index", j->st2);
-      launch_encode_filestats(mcols, W, nfiles, j->sms, j->st2);
-      launch_encode_index(mcols, ep, W, nblocks, nfiles, out_base_d, err, j->sms, j->st2, &launches);
+      launch_encode_filestats(mcols, W, nfiles, j->st2);
+      launch_encode_index(mcols, ep, W, nblocks, nfiles, out_base_d, j->sms, j->st2, &launches);
       j->kt_end(slot, j->st2);
     }
     CU(cudaEventRecord(j->evx[3], j->st2));
@@ -859,9 +845,8 @@ int encode_columns(b200c_job* j, uint64_t n, const void* pfx, const void* tr, co
 int run_merge_encode(b200c_job* j, int until, KeyCols decc, RunBounds runs, uint64_t n_decoded, uint64_t N, bool clipped,
                      uint64_t range_value_bytes, uint64_t* small, uint32_t* err, uint64_t launches);
 
-int run_job(b200c_job* j, int until) {
-  const b200c_params& P = j->p;
-  CU(cudaSetDevice(P.device));
+int job_prepare(b200c_job* j) {
+  CU(cudaSetDevice(j->p.device));
   if (!j->st) {
     CU(cudaStreamCreateWithFlags(&j->st, cudaStreamNonBlocking));
     {
@@ -872,18 +857,24 @@ int run_job(b200c_job* j, int until) {
     for (auto& e : j->ev) CU(cudaEventCreate(&e));
     for (auto& e : j->evx) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     cudaDeviceProp prop;
-    CU(cudaGetDeviceProperties(&prop, P.device));
+    CU(cudaGetDeviceProperties(&prop, j->p.device));
     j->sms = prop.multiProcessorCount;
   }
-  cudaStream_t st = j->st;
-  if (j->wait_ev) CU(cudaStreamWaitEvent(st, j->wait_ev, 0));  // sub-job of a range-pipelined parent: its part of the inputs is on its way
-  uint64_t launches = 0;
   j->outputs.clear();
   j->ran = false;
   j->stage_done = 0;
   j->kt_used = 0;
   j->pin_up_used = 0;
   memset(&j->stats, 0, sizeof j->stats);
+  return B200C_OK;
+}
+
+int run_job(b200c_job* j, int until) {
+  const b200c_params& P = j->p;
+  if (int rc = job_prepare(j)) return rc;
+  cudaStream_t st = j->st;
+  if (j->wait_ev) CU(cudaStreamWaitEvent(st, j->wait_ev, 0));  // sub-job of a range-pipelined parent: its part of the inputs is on its way
+  uint64_t launches = 0;
   const int k = (int)j->inputs.size();
   if (k == 0) return fail(B200C_ERR_INVALID_ARGUMENT, "job has no inputs");
 
@@ -1133,37 +1124,21 @@ int run_merge_encode(b200c_job* j, int until, KeyCols decc, RunBounds runs, uint
   W.tstat = j->tstat.as<TileStat>();
   W.min_s1 = reinterpret_cast<uint32_t*>(small + kSlotMinS1);
   W.totals = small + kSlotTotals;
-  bool unfolded = false;
   if (N) {
     j->kt_begin("merge.partition");
     launch_merge_partition(decc, runs, (uint32_t)k, N, mtiles, j->splits.as<uint64_t>(), err, j->sms, st);
     j->kt_end();
-    // the merge kernel also writes what the encoder needs per entry (encoded size, shared-prefix length) and per tile (statistics);
-    // B200C_MERGE_FOLD=0 keeps that in a pass of its own behind the merge (encode_sizes_kernel), for comparison
-    static const bool fold = !(getenv("B200C_MERGE_FOLD") && atoi(getenv("B200C_MERGE_FOLD")) == 0);
-    const MergeSizes msz = fold ? MergeSizes{W.esz, W.eshared, W.tstat, W.min_s1} : MergeSizes{nullptr, nullptr, nullptr, nullptr};
+    // the merge kernel also writes what the encoder needs per entry (encoded size, shared-prefix length) and per tile (statistics)
+    const MergeSizes msz{W.esz, W.eshared, W.tstat, W.min_s1};
     W.tprefix = j->tile_state.as<unsigned long long>();
     W.nstat = mtiles;
     j->kt_begin("merge.tiles");
     launch_merge_tiles(decc, runs, mp, N, mtiles, j->splits.as<uint64_t>(),
-                       j->tile_state.as<unsigned long long>(), reinterpret_cast<uint32_t*>(small + kSlotTicket), mrg, counters, msz, err, j->sms, st);
+                       j->tile_state.as<unsigned long long>(), reinterpret_cast<uint32_t*>(small + kSlotTicket), mrg, counters, msz, err, st);
     j->kt_end();
-    if (fold) {
-      j->kt_begin("merge.sizes_fix");
-      launch_merge_sizes_fix(KeyCols{mrg.pfx, mrg.tr, mrg.vref, mrg.meta, 0}, j->tile_state.as<unsigned long long>(), mtiles, msz, st);
-      j->kt_end();
-    } else {
-      CU(j->tprefix2.reserve(8 * (N / kEncTile + 2)));
-      CU(j->tstat.reserve(sizeof(TileStat) * (std::max<uint64_t>(mtiles, N / kEncTile) + 2)));
-      W.tstat = j->tstat.as<TileStat>();
-      W.tprefix = j->tprefix2.as<unsigned long long>();
-      W.nstat = 0;  // set below from the survivor count
-      j->kt_begin("encode.sizes");
-      launch_encode_sizes(KeyCols{mrg.pfx, mrg.tr, mrg.vref, mrg.meta, 0}, reinterpret_cast<const unsigned long long*>(&counters->n_out), W,
-                          j->tprefix2.as<unsigned long long>(), N, j->sms, st);
-      j->kt_end();
-      unfolded = true;
-    }
+    j->kt_begin("merge.sizes_fix");
+    launch_merge_sizes_fix(KeyCols{mrg.pfx, mrg.tr, mrg.vref, mrg.meta, 0}, j->tile_state.as<unsigned long long>(), mtiles, msz, st);
+    j->kt_end();
     launches += 3;
   }
   CU(cudaEventRecord(j->ev[2], st));
@@ -1180,7 +1155,6 @@ int run_merge_encode(b200c_job* j, int until, KeyCols decc, RunBounds runs, uint
   MergeCounters mc;
   memcpy(&mc, h + kSlotCounters, sizeof mc);
   const uint64_t n_out = mc.n_out;
-  if (unfolded) W.nstat = (n_out + kEncTile - 1) / kEncTile;  // statistics per kEncTile output entries (encode_sizes_kernel)
   j->n_out = n_out;
   mcols.n = n_out;
   j->stats.num_output_records = n_out;
@@ -1209,30 +1183,6 @@ int run_merge_encode(b200c_job* j, int until, KeyCols decc, RunBounds runs, uint
     if (rc) return rc;
   }
   return finish_run(j, launches, nblocks, nfiles);
-}
-
-int job_prepare(b200c_job* j) {
-  CU(cudaSetDevice(j->p.device));
-  if (!j->st) {
-    CU(cudaStreamCreateWithFlags(&j->st, cudaStreamNonBlocking));
-    {
-      int prio_lo = 0, prio_hi = 0;
-      CU(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
-      CU(cudaStreamCreateWithPriority(&j->st2, cudaStreamNonBlocking, prio_hi));
-    }
-    for (auto& e : j->ev) CU(cudaEventCreate(&e));
-    for (auto& e : j->evx) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    cudaDeviceProp prop;
-    CU(cudaGetDeviceProperties(&prop, j->p.device));
-    j->sms = prop.multiProcessorCount;
-  }
-  j->outputs.clear();
-  j->ran = false;
-  j->stage_done = 0;
-  j->kt_used = 0;
-  j->pin_up_used = 0;
-  memset(&j->stats, 0, sizeof j->stats);
-  return B200C_OK;
 }
 
 // TableBuilder side only: one sorted run given as device columns -> BlockBasedTable image(s)
@@ -1415,7 +1365,7 @@ int b200c_job_add_input(b200c_job* j, int level, uint64_t file_number, const voi
   in.data = static_cast<const uint8_t*>(data);
   in.len = len;
   in.mem_kind = mem_kind;
-  if (mem_kind == B200C_MEM_HOST && !deferred && len >= (1u << 20) && !getenv("B200C_NO_EAGER_UPLOAD")) {
+  if (mem_kind == B200C_MEM_HOST && !deferred && len >= (1u << 20)) {
     // Start the host -> device copy now, on the job's copy stream: a caller that reads its input files one after the other (the
     // executor plugin) gets the PCIe transfer of file i overlapped with the read of file i + 1.  Failures here are not errors: the
     // run copies the file itself when no eager copy is pending.
@@ -1655,7 +1605,7 @@ void b200c_job_destroy(b200c_job* j) {
   if (j->st) cudaStreamSynchronize(j->st);
   if (j->st2) cudaStreamSynchronize(j->st2);
   if (j->st_up) cudaStreamSynchronize(j->st_up);  // (an eager upload may also still be reading a caller's buffer)
-  DevBuf* all[] = {&j->files_d, &j->blk_off, &j->blk_size, &j->blk_state, &j->scan_tmp, &j->run_start, &j->run_bounds, &j->run_first_d, &j->kv_arena, &j->kv_offs, &j->kv_klens, &j->bloom_contrib, &j->bloom_contrib_off, &j->bloom_hashes, &j->tprefix2, &j->small,
+  DevBuf* all[] = {&j->files_d, &j->blk_off, &j->blk_size, &j->blk_state, &j->scan_tmp, &j->run_start, &j->run_bounds, &j->run_first_d, &j->kv_arena, &j->kv_offs, &j->kv_klens, &j->bloom_contrib, &j->bloom_contrib_off, &j->bloom_hashes, &j->small,
                    &j->dec[0], &j->dec[1], &j->dec[2], &j->dec[3], &j->mrg[0], &j->mrg[1], &j->mrg[2], &j->mrg[3], &j->splits,
                    &j->tile_state, &j->snaps_d, &j->esz, &j->eshared, &j->tstat, &j->nxt, &j->disk, &j->rows, &j->tstate, &j->grows, &j->gstate, &j->gflag, &j->gsync, &j->idx_contrib, &j->idx_contrib_off, &j->blocks,
                    &j->files_rec, &j->idx_esz, &j->idx_eoff, &j->idx_sep, &j->out_buf, &j->out_base_d};

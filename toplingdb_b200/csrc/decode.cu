@@ -737,8 +737,8 @@ __device__ __noinline__ void decode_block_slow(const uint8_t* p, uint32_t size, 
   }
 }
 
-template <int kMinCtas>
-__global__ void __launch_bounds__(kDecWarps * 32, kMinCtas)
+constexpr int kDecCtasPerSm = 4;  // 64 registers (a small spill), but 32 independent warps per SM
+__global__ void __launch_bounds__(kDecWarps * 32, kDecCtasPerSm)
 block_decode_fused_kernel(const FileDesc* __restrict__ files, int nfiles, const uint64_t* __restrict__ blk_off,
                           const uint32_t* __restrict__ blk_size, uint32_t nblk, uint32_t verify, uint64_t n_total, KeyColsMut out,
                           unsigned long long* blk_state, uint32_t* ticket, uint64_t* __restrict__ run_start,
@@ -1002,20 +1002,19 @@ void launch_index_decode(const FileDesc* files_dev, int nfiles, uint32_t max_blo
 void launch_block_decode_fused(const FileDesc* files_dev, int nfiles, const uint64_t* blk_off, const uint32_t* blk_size, uint32_t nblk,
                                uint32_t verify, uint64_t n_total, KeyColsMut out, unsigned long long* blk_state, uint32_t* ticket,
                                uint64_t* run_start, uint64_t* total_out, uint32_t* err, int sms, cudaStream_t st, const uint8_t* arena) {
-  constexpr int kCtasPerSm = 4;  // 64 registers (a small spill), but 32 independent warps per SM
   const int smem = kDecWarps * (int)sizeof(DecWarpSmem);
-  static_assert(kCtasPerSm * (kDecWarps * sizeof(DecWarpSmem) + 4096) <= 227 * 1024, "four decode CTAs must fit one SM");
+  static_assert(kDecCtasPerSm * (kDecWarps * sizeof(DecWarpSmem) + 4096) <= 227 * 1024, "four decode CTAs must fit one SM");
   static PerDeviceFlag attr;
   const uint64_t dev_bit = attr.bit_of_current_device();
   if (!attr.is_set(dev_bit)) {
-    cudaFuncSetAttribute(block_decode_fused_kernel<kCtasPerSm>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaFuncSetAttribute(block_decode_fused_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     attr.set(dev_bit);
   }
   const unsigned per = kDecWarps;
-  unsigned want = (nblk + per - 1) / per, cap = (unsigned)sms * (unsigned)kCtasPerSm;
+  unsigned want = (nblk + per - 1) / per, cap = (unsigned)sms * (unsigned)kDecCtasPerSm;
   const unsigned grid = want < cap ? (want ? want : 1) : cap;
-  block_decode_fused_kernel<kCtasPerSm><<<grid, kDecWarps * 32, smem, st>>>(files_dev, nfiles, blk_off, blk_size, nblk, verify, n_total, out,
-                                                                             blk_state, ticket, run_start, total_out, err, arena);
+  block_decode_fused_kernel<<<grid, kDecWarps * 32, smem, st>>>(files_dev, nfiles, blk_off, blk_size, nblk, verify, n_total, out,
+                                                                 blk_state, ticket, run_start, total_out, err, arena);
 }
 void launch_gather_values(KeyCols in, const uint64_t* dst_off, uint8_t* dst, cudaStream_t st) {
   if (in.n == 0) return;

@@ -8,7 +8,7 @@
 //
 // The reference cuts blocks with a sequential greedy rule.  Here it is evaluated in parallel:
 //   encode_sizes      per entry: shared-prefix length with the previous internal key and encoded size; per tile: partial
-//                     sums for the per-file statistics
+//                     sums for the per-file statistics (TableBuilder path only: a compaction's merge kernel writes these)
 //   encode_tables     per tile of kEncTile entries: next(a) = "where does a block that starts at entry a end" for every
 //                     a (prefix sums + bisection in shared memory), then the tile's transfer function
 //                     entry-point -> (exit point, bytes, #blocks) for every entry point a chain can arrive at
@@ -19,8 +19,6 @@
 //                     into a shared-memory image, restart array, checksum, coalesced store into the file image
 //   encode_index_*    per block separator keys, per-file index block, its checksum
 // HBM-bound; algorithmic bytes of encode_emit = 36 B of columns + value bytes read + block bytes written per entry.
-#include <cstdlib>
-
 #include "bloom_rules.h"
 #include "common.cuh"
 #include "gp_rules.h"
@@ -34,8 +32,9 @@ constexpr int kW = kEncTile + kEncHalo;
 constexpr int kEncThreads = 256;
 
 // ------------------------------------------------------------------------------------------------ entry sizes
-// (ikey_byte / shared_prefix / entry_size live in common.cuh: the merge kernel writes the sizes of the entries it emits)
-// One CTA per tile of kEncTile merged entries (grid-stride over tiles): shared-prefix length + encoded size of every entry, the
+// (ikey_byte / shared_prefix / entry_size live in common.cuh: the merge kernel writes the sizes of the entries it emits, so this
+// pass serves the TableBuilder path, which has no merge in front of it)
+// One CTA per tile of kEncTile sorted entries (grid-stride over tiles): shared-prefix length + encoded size of every entry, the
 // global min / max entry size, and the tile's partial sums for the per-file statistics (so that the statistics pass reads
 // 40 bytes per tile instead of 12 bytes per entry).
 __global__ void __launch_bounds__(256)
@@ -790,17 +789,8 @@ encode_stitch_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t n, uint
     s.gn = s.tn = 0;
   }
   __syncthreads();
-#ifdef B200C_STITCH_TRACE
-  long long tr_walk = 0, tr_wait = 0, tr_ref2 = 0, tr_ref3 = 0, tr_chase = 0, tr_n2 = 0, tr_n3 = 0, tr_nc = 0, tr_t = 0;
-#define TR_BEGIN() (tr_t = clock64())
-#define TR_END(acc) ((acc) += clock64() - tr_t)
-#else
-#define TR_BEGIN() ((void)0)
-#define TR_END(acc) ((void)0)
-#endif
   for (;;) {
     if (threadIdx.x == 0) {
-      TR_BEGIN();
       // everything the serial walk touches per step lives in registers; shared memory is read / written once per section
       WalkState st = s.st;
       const GpState gps = s.gp;  // only read here: boundaries are crossed (and the state changes) inside chase_tile
@@ -886,7 +876,6 @@ encode_stitch_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t n, uint
       s.req = req;
       s.req_idx = req_idx;
       if (fin) s.done = 1;
-      TR_END(tr_walk);
     }
     __syncthreads();
     const uint32_t req = s.req;  // stable: thread 0 writes these again only after the barrier that ends the iteration
@@ -899,7 +888,6 @@ encode_stitch_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t n, uint
       if (req == 2) {
         // the tables kernel is still running: wait for the first group needed, then take the consecutive groups that are ready too
         if (threadIdx.x == 0) {
-          TR_BEGIN();
           volatile uint32_t* rdy = wk.gready;
           if (first_wait) {
             unsigned long long t0, t1;
@@ -915,7 +903,6 @@ encode_stitch_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t n, uint
           } else {
             while (rdy[ridx] == 0) __nanosleep(256);
           }
-          TR_END(tr_wait);
           uint32_t have = 1;
           while (have < cnt && rdy[ridx + have] != 0) have++;
           s.refill = have;
@@ -929,11 +916,7 @@ encode_stitch_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t n, uint
       // tile rows (req == 3) belong to a group that was ready when its row entered the group cache
       const uint4* src = reinterpret_cast<const uint4*>((req == 2 ? wk.grows : wk.rows) + ridx * hc);
       uint4* dst = reinterpret_cast<uint4*>(req == 2 ? gcache : tcache);
-      TR_BEGIN();
       coop_copy_cg<uint4, 8>(dst, src, cnt * hc);
-#ifdef B200C_STITCH_TRACE
-      if (req == 2) { TR_END(tr_ref2); tr_n2++; } else { TR_END(tr_ref3); tr_n3++; }
-#endif
       if (threadIdx.x == 0) {
         if (req == 2) {
           s.ga = ridx;
@@ -946,7 +929,6 @@ encode_stitch_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t n, uint
     } else if (req == 1) {
       const uint64_t tstart = ridx * (uint64_t)kTT;
       const uint32_t tl = (uint32_t)(((tstart + kTT) < n ? (tstart + kTT) : n) - tstart);
-      TR_BEGIN();
       // only the part of the tile the chain can still touch: from the walk's position on (16-byte vectors: the tile starts are
       // multiples of kTT, so element c0 = position rounded down to 8 is 16-byte aligned in both arrays)
       const uint32_t c0 = (uint32_t)(s.st.a > tstart ? (s.st.a - tstart) & ~7ull : 0);
@@ -1012,21 +994,11 @@ encode_stitch_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t n, uint
         s.st = st;
       }
       __syncthreads();
-#ifdef B200C_STITCH_TRACE
-      TR_END(tr_chase);
-      tr_nc++;
-#endif
       done = s.done;
     }
     __syncthreads();
     if (done) break;
   }
-#ifdef B200C_STITCH_TRACE
-  if (threadIdx.x == 0) {
-    wk.totals[16] = tr_walk, wk.totals[17] = tr_wait, wk.totals[18] = tr_ref2, wk.totals[19] = tr_ref3, wk.totals[20] = tr_chase;
-    wk.totals[21] = tr_n2, wk.totals[22] = tr_n3, wk.totals[23] = tr_nc;
-  }
-#endif
   if (threadIdx.x == 0) {
     wk.totals[0] = s.st.blk;
     wk.totals[1] = s.st.f;
@@ -1408,11 +1380,6 @@ __device__ void emit_block_warp(const KeyCols& m, const EncodeParams& ep, const 
   }
 }
 
-// Batched emit: a CTA takes kEmitBatch consecutive data blocks.  Their entries are consecutive in the merged stream, so
-// every thread owns a few entries, loads their columns with coalesced accesses and their values with independent
-// aligned word loads (everything in flight at once: one memory latency per batch instead of one per 32 entries),
-// a CTA-wide scan turns entry sizes into byte offsets, threads write their entries into the block images in shared
-// memory, then one warp per block adds restart footer + checksum trailer and stores the image.
 // internal key bytes [sh, sh + n) (n <= 24) as three little-endian words, from the columnar (hi, lo, ulen, trailer) form
 __device__ __forceinline__ void key_suffix_words(uint64_t hi, uint64_t lo, uint32_t ulen, uint64_t tr, uint32_t sh, uint64_t* S0,
                                                  uint64_t* S1, uint64_t* S2) {
@@ -2525,8 +2492,6 @@ void launch_encode_tables(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nti
 void launch_encode_stitch(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t ntiles, uint32_t hc, uint32_t* err, uint32_t attempt,
                           uint32_t* sflag, cudaStream_t st, uint64_t* launches) {
   if (ntiles == 0) return;
-  static const bool solo = !(getenv("B200C_STITCH_SOLO") && atoi(getenv("B200C_STITCH_SOLO")) == 0);  // 0: only the launch behind the tables kernel
-  if (attempt == 1 && !solo) return;
   static PerDeviceFlag attr;
   const uint64_t dev_bit = attr.bit_of_current_device();
   constexpr size_t kSolo = 200 * 1024;  // attempt 1: no tables CTA (>= 60 KB of shared memory) fits next to it
@@ -2559,9 +2524,8 @@ void launch_encode_blocklist(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t 
   if (ntiles == 0) return;
   encode_blocklist_kernel<<<(unsigned)ntiles, kEncThreads, 0, st>>>(m, ep, w, m.n, nblk_cap, err);
 }
-void launch_encode_filestats(KeyCols m, EncodeWork w, uint32_t nfiles, int sms, cudaStream_t st) {
+void launch_encode_filestats(KeyCols m, EncodeWork w, uint32_t nfiles, cudaStream_t st) {
   if (m.n == 0 || nfiles == 0) return;
-  (void)sms;
   encode_filestats_kernel<<<nfiles, 256, 0, st>>>(m, w, nfiles);
 }
 constexpr uint32_t kEmitMaxSmem = 224 * 1024;  // dynamic shared memory of one emit CTA at most (+ ~2 KB static: XXH3 lane table, mbarriers)
@@ -2606,8 +2570,7 @@ void launch_encode_emit(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nbloc
   else encode_emit_kernel<<<grid, warps * 32, smem, st>>>(m, ep, w, nblocks, out_base, slot, err);
 }
 void launch_encode_index(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nblocks, uint32_t nfiles, uint8_t* const* out_base,
-                         uint32_t* err, int sms, cudaStream_t st, uint64_t* launches) {
-  (void)err;
+                         int sms, cudaStream_t st, uint64_t* launches) {
   if (nblocks == 0) return;
   unsigned g = (unsigned)((nblocks + 255) / 256);
   if (g > (unsigned)sms * 8) g = (unsigned)sms * 8;

@@ -132,7 +132,7 @@ void launch_merge_partition(KeyCols in, RunBounds runs, uint32_t nruns, uint64_t
                             uint64_t* splits, uint32_t* err, int sms, cudaStream_t st);
 void launch_merge_tiles(KeyCols in, RunBounds runs, MergeParams mp, uint64_t n_total, uint64_t ntiles,
                         const uint64_t* splits, unsigned long long* tile_state, uint32_t* ticket, KeyColsMut out,
-                        MergeCounters* counters, MergeSizes ms, uint32_t* err, int sms, cudaStream_t st);
+                        MergeCounters* counters, MergeSizes ms, uint32_t* err, cudaStream_t st);
 // sizes of each tile's first output entry (needs the finished tile_state prefixes and merged columns)
 void launch_merge_sizes_fix(KeyCols merged, const unsigned long long* tile_state, uint64_t ntiles, MergeSizes ms, cudaStream_t st);
 
@@ -240,13 +240,13 @@ void launch_encode_stitch(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nti
 void launch_encode_tilestate(KeyCols m, EncodeWork w, uint64_t ntiles, uint32_t hc, uint32_t* err, cudaStream_t st, uint64_t* launches);
 void launch_encode_blocklist(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t ntiles, uint64_t nblk_cap, uint32_t* err,
                              cudaStream_t st);
-void launch_encode_filestats(KeyCols m, EncodeWork w, uint32_t nfiles, int sms, cudaStream_t st);
+void launch_encode_filestats(KeyCols m, EncodeWork w, uint32_t nfiles, cudaStream_t st);
 uint32_t encode_emit_slice(uint32_t block_size);
 // out_base[f] = device address where file f's image starts; data_bytes = all data blocks incl. trailers (with m.n: selects the kernel)
 void launch_encode_emit(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nblocks, uint8_t* const* out_base, uint64_t data_bytes,
                         uint32_t* err, int sms, cudaStream_t st);
 void launch_encode_index(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nblocks, uint32_t nfiles, uint8_t* const* out_base,
-                         uint32_t* err, int sms, cudaStream_t st, uint64_t* launches);
+                         int sms, cudaStream_t st, uint64_t* launches);
 void launch_block_checksums(uint32_t type, const uint8_t* data, const uint64_t* offsets, uint32_t n, uint8_t last_byte,
                             uint32_t* out, cudaStream_t st);
 

@@ -14,8 +14,6 @@
 //                           output offset (count published early, offset resolved after the value-reference gathers),
 //                           coalesced write of the surviving (key, value-ref) records.
 // HBM-bound: algorithmic bytes = 36 B read per input entry + 36 B written per surviving entry.
-#include <cstdlib>
-
 #include "common.cuh"
 #include "group_rules.h"
 #include "kernels.h"
@@ -218,10 +216,7 @@ __device__ __forceinline__ void msel_grouped(const KeyCols& in, const GroupLanes
 // 12 CTAs (48 warps) per SM: 42 registers with a small spill, but all of a job's warps are resident at once -- the kernel is one
 // chain of dependent loads per warp, so residency is what counts (faster on cfg2 than the 64 registers ptxas takes unasked, or than
 // 10 CTAs).
-#ifndef B200C_PART_MIN_CTAS
-#define B200C_PART_MIN_CTAS 12
-#endif
-__global__ void __launch_bounds__(128, B200C_PART_MIN_CTAS)
+__global__ void __launch_bounds__(128, 12)
 merge_partition_grouped_kernel(KeyCols in, RunBounds runs, uint32_t nruns, uint32_t gshift, uint64_t n_total,
                                uint64_t ntiles, uint64_t* __restrict__ splits, uint32_t* __restrict__ err, uint32_t chunk) {
   const unsigned lane = threadIdx.x & 31;
@@ -555,14 +550,16 @@ __device__ __noinline__ void sd_walk_tile(TileSmem& s, const KeyCols& in, const 
   __syncthreads();
 }
 
+// three CTAs per SM at 80 registers (four at 64 registers, with spills, were slower)
+constexpr int kMergeCtasPerSm = 3;
 // kSD: the variant for jobs whose inputs hold a kTypeSingleDeletion (the decoder notes that in the error word).  Both variants are
 // launched; the one that does not apply leaves at once.  Keeping the serial walk and its bookkeeping out of the common variant
 // shortens the common case.
-template <int kMinCtas, bool kSD>
-__global__ void __launch_bounds__(kMThreads, kMinCtas)
+template <bool kSD>
+__global__ void __launch_bounds__(kMThreads, kMergeCtasPerSm)
 merge_tiles_kernel(KeyCols in, RunBounds runs, MergeParams mp, uint64_t n_total, uint64_t ntiles,
                    const uint64_t* __restrict__ splits, unsigned long long* tile_state, uint32_t* ticket, KeyColsMut out,
-                   MergeCounters* counters, MergeSizes ms, uint32_t* __restrict__ err, uint32_t prefetch_dist) {
+                   MergeCounters* counters, MergeSizes ms, uint32_t* __restrict__ err) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   TileSmem& s = *reinterpret_cast<TileSmem*>(smem_raw);
   const uint32_t t = threadIdx.x, lane = t & 31, w = t >> 5;
@@ -957,7 +954,6 @@ merge_tiles_kernel(KeyCols in, RunBounds runs, MergeParams mp, uint64_t n_total,
     }
     __syncthreads();
     const uint64_t base_out = s.base_out;
-    const bool fold = ms.esz != nullptr;  // the merge also writes the encoder's per-entry sizes and per-tile statistics
     // per-thread partial statistics of the output entries (TileStat) and entry-size extremes
     uint32_t st_kb = 0, st_nd = 0, mn = 0xffffffffu, mx = 0;
     unsigned long long st_vb = 0, st_smin = ~0ull, st_smax = 0;
@@ -975,7 +971,7 @@ merge_tiles_kernel(KeyCols in, RunBounds runs, MergeParams mp, uint64_t n_total,
         out.meta[dst] = gm[j];
         // encoded size against the previous OUTPUT entry (BlockBuilder::AddWithLastKey); the tile's first entry is left to
         // merge_sizes_fix_kernel: its predecessor is the last survivor of an earlier tile
-        if (fold && i > 0) {
+        if (i > 0) {
           const uint32_t pp = s.idx[PH(i - 1)];
           const uint32_t sh = shared_prefix(chi, clo, cul, ctr, s.hi[pp], s.lo[pp], s.ulen[pp] & 0x3fu, s.tr[pp]);
           const uint32_t s1 = entry_size(sh, cul + 8, vlen);
@@ -992,26 +988,24 @@ merge_tiles_kernel(KeyCols in, RunBounds runs, MergeParams mp, uint64_t n_total,
         st_smax = sq > st_smax ? sq : st_smax;
       }
     }
-    if (fold) {
-      const unsigned kb = __reduce_add_sync(0xffffffffu, st_kb), nd = __reduce_add_sync(0xffffffffu, st_nd);
-      mn = __reduce_min_sync(0xffffffffu, mn);
-      mx = __reduce_max_sync(0xffffffffu, mx);
+    const unsigned kb = __reduce_add_sync(0xffffffffu, st_kb), nd = __reduce_add_sync(0xffffffffu, st_nd);
+    mn = __reduce_min_sync(0xffffffffu, mn);
+    mx = __reduce_max_sync(0xffffffffu, mx);
 #pragma unroll
-      for (int dd = 16; dd; dd >>= 1) {
-        st_vb += __shfl_xor_sync(0xffffffffu, st_vb, dd);
-        const unsigned long long a = __shfl_xor_sync(0xffffffffu, st_smin, dd), b = __shfl_xor_sync(0xffffffffu, st_smax, dd);
-        st_smin = a < st_smin ? a : st_smin;
-        st_smax = b > st_smax ? b : st_smax;
-      }
-      if (lane == 0) {
-        atomicAdd(&s.stat[0], (unsigned long long)kb);
-        atomicAdd(&s.stat[1], st_vb);
-        atomicAdd(&s.stat[2], (unsigned long long)nd);
-        atomicMin(&s.stat[3], st_smin);
-        atomicMax(&s.stat[4], st_smax);
-        atomicMin(&s.smin, mn);
-        atomicMax(&s.smax, mx);
-      }
+    for (int dd = 16; dd; dd >>= 1) {
+      st_vb += __shfl_xor_sync(0xffffffffu, st_vb, dd);
+      const unsigned long long a = __shfl_xor_sync(0xffffffffu, st_smin, dd), b = __shfl_xor_sync(0xffffffffu, st_smax, dd);
+      st_smin = a < st_smin ? a : st_smin;
+      st_smax = b > st_smax ? b : st_smax;
+    }
+    if (lane == 0) {
+      atomicAdd(&s.stat[0], (unsigned long long)kb);
+      atomicAdd(&s.stat[1], st_vb);
+      atomicAdd(&s.stat[2], (unsigned long long)nd);
+      atomicMin(&s.stat[3], st_smin);
+      atomicMax(&s.stat[4], st_smax);
+      atomicMin(&s.smin, mn);
+      atomicMax(&s.smax, mx);
     }
   }
   // ---- counters: one atomic per CTA and counter.  Per-thread partial counts are small (<= kMV entries), so the warp
@@ -1037,7 +1031,7 @@ merge_tiles_kernel(KeyCols in, RunBounds runs, MergeParams mp, uint64_t n_total,
   }
   __syncthreads();
   if (t < 8 && s.red[t]) atomicAdd(((unsigned long long*)counters) + t, s.red[t]);
-  if (t == 0 && ms.esz != nullptr) {
+  if (t == 0) {
     ms.tstat[tile] = TileStat{s.stat[0], s.stat[1], s.stat[2], s.stat[3], s.stat[4]};
     if (s.smin != 0xffffffffu) {
       atomicMin(ms.min_s1, s.smin);
@@ -1150,13 +1144,10 @@ void launch_merge_partition(KeyCols in, RunBounds runs, uint32_t nruns, uint64_t
     while (kp2 < nruns) kp2 <<= 1;
     uint32_t gshift = 0;
     while ((kp2 << (gshift + 1)) <= 32) gshift++;  // lanes per run = 32 / pow2(nruns)
-    static const uint32_t chunk_env = getenv("B200C_PART_CHUNK") ? (uint32_t)atoi(getenv("B200C_PART_CHUNK")) : 0;  // tuning knob
-    uint32_t chunk = chunk_env;
-    if (chunk == 0) {  // about one and a half waves of warps (32 resident per SM at 64 registers)
-      const unsigned wave = (unsigned)sms * 48u;
-      chunk = (uint32_t)((warps + wave - 1) / wave);
-      if (chunk > 4) chunk = 4;
-    }
+    // about one and a half waves of warps (32 resident per SM at 64 registers)
+    const unsigned wave = (unsigned)sms * 48u;
+    uint32_t chunk = (uint32_t)((warps + wave - 1) / wave);
+    if (chunk > 4) chunk = 4;
     if (chunk < 1) chunk = 1;
     const unsigned chunks = (warps + chunk - 1) / chunk;
     merge_partition_grouped_kernel<<<(chunks + 3) / 4, 128, 0, st>>>(in, runs, nruns, gshift, n_total, ntiles, splits, err, chunk);
@@ -1165,23 +1156,22 @@ void launch_merge_partition(KeyCols in, RunBounds runs, uint32_t nruns, uint64_t
   merge_partition_kernel<<<(warps + 3) / 4, 128, 0, st>>>(in, runs, nruns, n_total, ntiles, splits, err);
 }
 static_assert(sizeof(Key) * kMaxRuns <= sizeof(uint64_t) * kMT && 4 * kMaxRuns <= 2 * kMT, "candidate staging must fit");
-static_assert(3 * (sizeof(TileSmem) + 1024) <= 227 * 1024, "merge tile must fit three CTAs per SM");
+static_assert(kMergeCtasPerSm * (sizeof(TileSmem) + 1024) <= 227 * 1024, "merge tile must fit three CTAs per SM");
 void launch_merge_tiles(KeyCols in, RunBounds runs, MergeParams mp, uint64_t n_total, uint64_t ntiles,
                         const uint64_t* splits, unsigned long long* tile_state, uint32_t* ticket, KeyColsMut out,
-                        MergeCounters* counters, MergeSizes ms, uint32_t* err, int sms, cudaStream_t st) {
+                        MergeCounters* counters, MergeSizes ms, uint32_t* err, cudaStream_t st) {
   if (ntiles == 0) return;
   static PerDeviceFlag attr;
   const uint64_t dev_bit = attr.bit_of_current_device();
   if (!attr.is_set(dev_bit)) {
-    cudaFuncSetAttribute(merge_tiles_kernel<3, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileSmem));
-    cudaFuncSetAttribute(merge_tiles_kernel<3, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileSmem));
+    cudaFuncSetAttribute(merge_tiles_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileSmem));
+    cudaFuncSetAttribute(merge_tiles_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(TileSmem));
     attr.set(dev_bit);
   }
-  // three CTAs per SM at 80 registers (four at 64 registers, with spills, were slower)
-  merge_tiles_kernel<3, false><<<(unsigned)ntiles, kMThreads, sizeof(TileSmem), st>>>(in, runs, mp, n_total, ntiles, splits, tile_state, ticket,
-                                                                                      out, counters, ms, err, (unsigned)sms * 3u);
-  merge_tiles_kernel<3, true><<<(unsigned)ntiles, kMThreads, sizeof(TileSmem), st>>>(in, runs, mp, n_total, ntiles, splits, tile_state, ticket,
-                                                                                     out, counters, ms, err, (unsigned)sms * 3u);
+  merge_tiles_kernel<false><<<(unsigned)ntiles, kMThreads, sizeof(TileSmem), st>>>(in, runs, mp, n_total, ntiles, splits, tile_state, ticket,
+                                                                                   out, counters, ms, err);
+  merge_tiles_kernel<true><<<(unsigned)ntiles, kMThreads, sizeof(TileSmem), st>>>(in, runs, mp, n_total, ntiles, splits, tile_state, ticket,
+                                                                                  out, counters, ms, err);
 }
 void launch_merge_sizes_fix(KeyCols merged, const unsigned long long* tile_state, uint64_t ntiles, MergeSizes ms, cudaStream_t st) {
   if (ntiles) merge_sizes_fix_kernel<<<(unsigned)((ntiles + 127) / 128), 128, 0, st>>>(merged, tile_state, ntiles, ms);
