@@ -492,6 +492,7 @@ struct XxhLaneTab {
   uint64_t kscr[32];   // scramble secret
   uint64_t klast[32];  // secret of the last stripe
   uint64_t kmrg[32];   // merge secret
+  uint64_t kinit[32];  // initial value of the lane's accumulator
 };
 
 // ---- mbarrier + TMA bulk copy (global -> shared), sm_90+ ----------------------------------------------------------------------
@@ -542,6 +543,8 @@ __device__ __forceinline__ void fill_xxh_lane_tab(XxhLaneTab* t) {
     t->kscr[i] = sec64g(192 - 64 + 8 * a);
     t->klast[i] = sec64g(192 - 64 - 7 + 8 * a);
     t->kmrg[i] = sec64g(11 + 8 * a);
+    const uint64_t init[8] = {kP32_3, kP64_1, kP64_2, kP64_3, kP64_4, kP32_2, kP64_5, kP32_1};
+    t->kinit[i] = init[a];
   }
 }
 // 8 bytes at shared address p; o = p & 7 is the same for every lane (kPhase: 0 aligned, 1 o in 1..3, 2 o in 4..7)
@@ -561,11 +564,8 @@ __device__ __forceinline__ uint64_t lds64_phase(uint32_t p, uint32_t o) {
 template <int kPhase>
 __device__ __forceinline__ uint64_t xxh3_staged_t(uint32_t sp, uint32_t len, uint32_t tab, unsigned lane) {
   const uint32_t a = lane & 7, g = lane >> 3, o = sp & 7;
-  const uint64_t init[8] = {kP32_3, kP64_1, kP64_2, kP64_3, kP64_4, kP32_2, kP64_5, kP32_1};
-  uint64_t acc = init[0];
-#pragma unroll
-  for (int i = 1; i < 8; i++) acc = a == (uint32_t)i ? init[i] : acc;
   const uint32_t tl = tab + 8 * lane;  // this lane's column of the table
+  uint64_t acc = lds64(tl + 1792);     // (from the table: selecting it from a constant array put the array in local memory)
   const uint64_t k0 = lds64(tl), k1 = lds64(tl + 256), k2 = lds64(tl + 512), k3 = lds64(tl + 768), kscr = lds64(tl + 1024);
   const uint32_t nb_blocks = (len - 1) >> 10;
   uint32_t p = sp + 64 * g + 8 * a;  // stripe g of the current 1024-byte block, this lane's word
@@ -615,7 +615,7 @@ __device__ __forceinline__ uint64_t xxh3_staged_t(uint32_t sp, uint32_t len, uin
   return xxh3_avalanche((uint64_t)len * kP64_1 + m);  // lanes 0..7 of a group hold the sum; every lane with a == 0..7 has it after the xors
 }
 static_assert(offsetof(XxhLaneTab, k) == 0 && offsetof(XxhLaneTab, kscr) == 1024 && offsetof(XxhLaneTab, klast) == 1280 &&
-                  offsetof(XxhLaneTab, kmrg) == 1536,
+                  offsetof(XxhLaneTab, kmrg) == 1536 && offsetof(XxhLaneTab, kinit) == 1792,
               "xxh3_staged_t addresses the lane table by these offsets");
 // block checksum (table/format.cc:468-509) of the staged block: type 4 = XXH3, 1 = CRC32C
 __device__ __forceinline__ uint32_t staged_block_checksum(uint32_t type, uint32_t sp, const uint8_t* p, uint32_t n, uint8_t last_byte, uint32_t xtab,
