@@ -76,26 +76,6 @@ __device__ __forceinline__ uint64_t ld_u64_funnel(const uint8_t* p) {
   if (a == 0) return lo;
   return (lo >> (8 * a)) | (q[1] << (64 - 8 * a));
 }
-// bytes [s, s+16) of the 32-byte concatenation A|B (s in 0..15, warp-uniform): re-aligns 16-byte vectors on the fly
-__device__ __forceinline__ uint4 shift16(uint4 A, uint4 B, uint32_t s) {
-  const uint32_t bs = (s & 3) * 8;
-  uint4 r;
-  switch (s >> 2) {
-    case 0:
-      r.x = __funnelshift_r(A.x, A.y, bs), r.y = __funnelshift_r(A.y, A.z, bs), r.z = __funnelshift_r(A.z, A.w, bs), r.w = __funnelshift_r(A.w, B.x, bs);
-      break;
-    case 1:
-      r.x = __funnelshift_r(A.y, A.z, bs), r.y = __funnelshift_r(A.z, A.w, bs), r.z = __funnelshift_r(A.w, B.x, bs), r.w = __funnelshift_r(B.x, B.y, bs);
-      break;
-    case 2:
-      r.x = __funnelshift_r(A.z, A.w, bs), r.y = __funnelshift_r(A.w, B.x, bs), r.z = __funnelshift_r(B.x, B.y, bs), r.w = __funnelshift_r(B.y, B.z, bs);
-      break;
-    default:
-      r.x = __funnelshift_r(A.w, B.x, bs), r.y = __funnelshift_r(B.x, B.y, bs), r.z = __funnelshift_r(B.y, B.z, bs), r.w = __funnelshift_r(B.z, B.w, bs);
-  }
-  return r;
-}
-
 __device__ __forceinline__ void prefetch_l2(const void* p) { asm volatile("prefetch.global.L2 [%0];" ::"l"(p)); }
 __device__ __forceinline__ void prefetch_l1(const void* p) { asm volatile("prefetch.global.L1 [%0];" ::"l"(p)); }
 
@@ -135,6 +115,19 @@ __host__ __device__ __forceinline__ int put_varint(uint8_t* p, uint64_t v) {
   }
   p[n++] = (uint8_t)v;
   return n;
+}
+// little-endian 32-bit store at any alignment (EncodeFixed32)
+__device__ __forceinline__ void put_fixed32(uint8_t* p, uint32_t v) {
+  p[0] = (uint8_t)v;
+  p[1] = (uint8_t)(v >> 8);
+  p[2] = (uint8_t)(v >> 16);
+  p[3] = (uint8_t)(v >> 24);
+}
+// 5-byte block trailer behind a block's contents: compression type kNoCompression + checksum (WriteMaybeCompressedBlock,
+// block_based_table_builder.cc:1305-1329)
+__device__ __forceinline__ void put_block_trailer(uint8_t* p, uint32_t cksum) {
+  p[0] = 0;
+  put_fixed32(p + 1, cksum);
 }
 
 // ---- key order (BytewiseCompareInternalKey, db/dbformat.h:1057-1097) ---------------------------------------

@@ -181,7 +181,6 @@ struct FileRec {             // one output file (device-computed part)
   uint64_t smallest_seq, largest_seq;
   KeyRec smallest, largest;
   uint32_t index_has_seq;    // some adjacent blocks share a user key => index keys keep the 8-byte trailer
-  uint32_t index_cksum;      // checksum word of the index block trailer
   uint64_t filter_entries;   // hashes in the Bloom filter (rocksdb.num.filter_entries); 0 without a filter policy
   uint64_t filter_bytes;     // filter block on disk: bits + 5 metadata bytes + 5 trailer bytes; sits between data and index blocks
 };
