@@ -493,14 +493,16 @@ int upload_small(b200c_job* j, void* dev_dst, const void* host_src, size_t n) {
 // Small device -> host reads (counters, per-file records) go through a tiny kernel that writes mapped pinned memory, not
 // through cudaMemcpy: a D2H copy would queue on the copy engine behind the multi-GB output downloads of OTHER jobs running
 // on the same device, and every host decision point of this job would wait for them.
-// Copies the `small` slots and (files != nullptr) the first *nfiles_dev file records, then synchronises the stream.
+// gather_small() enqueues the copy of the `small` slots and (files != nullptr) the first *nfiles_dev file records; take_small() reads
+// them once the stream has passed that point.  read_small() does both around a synchronisation of the stream.
 constexpr size_t kRdSmall = kSmallSlots * 8;
-int read_small(b200c_job* j, uint64_t* h, const FileRec* files = nullptr, std::vector<FileRec>* frs = nullptr) {
+int gather_small(b200c_job* j, const FileRec* files) {
   const uint64_t* small = j->small.as<uint64_t>();
   CU(j->pin_rd.reserve(kRdSmall + sizeof(FileRec) * (size_t)kMaxOutFiles));
   launch_gather_small(small, (uint32_t)kRdSmall, files, files ? small + kSlotTotals + 1 : nullptr, j->pin_rd.p, j->st);
-  CU(cudaStreamSynchronize(j->st));
-  CU(cudaGetLastError());
+  return B200C_OK;
+}
+void take_small(b200c_job* j, uint64_t* h, const FileRec* files, std::vector<FileRec>* frs) {
   memcpy(h, j->pin_rd.p, kRdSmall);
   if (files && frs) {
     uint64_t n = h[kSlotTotals + 1];
@@ -508,6 +510,12 @@ int read_small(b200c_job* j, uint64_t* h, const FileRec* files = nullptr, std::v
     frs->resize(n);
     memcpy(frs->data(), j->pin_rd.p + kRdSmall, sizeof(FileRec) * n);
   }
+}
+int read_small(b200c_job* j, uint64_t* h, const FileRec* files = nullptr, std::vector<FileRec>* frs = nullptr) {
+  if (int rc = gather_small(j, files)) return rc;
+  CU(cudaStreamSynchronize(j->st));
+  CU(cudaGetLastError());
+  take_small(j, h, files, frs);
   return B200C_OK;
 }
 // read_small() and then the error word the kernels raised: the checked synchronisation point between two stages
@@ -516,12 +524,12 @@ int checked_sync(b200c_job* j, uint64_t* h, const FileRec* files = nullptr, std:
   return map_dev_err((uint32_t)h[kSlotErr]);
 }
 
-// the tails of the outputs (properties, metaindex, footer) and their metas: built on the host, written into the images by one launch
+// the tails of the outputs (properties, metaindex, footer) and their metas: built on the host, written into the images by one launch.
+// pin_tails (4096 bytes per file) and pin_small (the TailCopy records) are reserved by encode_stage before the emit kernel starts.
 int write_tails(b200c_job* j, const std::vector<FileRec>& frs, const std::vector<uint64_t>& base_off) {
   const b200c_params& P = j->p;
   const uint32_t nfiles = (uint32_t)frs.size();
   j->outputs.resize(nfiles);
-  CU(j->pin_tails.reserve((size_t)nfiles * 4096 + 64));
   std::vector<TailCopy> tcs(nfiles);
   for (uint32_t f = 0; f < nfiles; f++) {
     const FileRec& fr = frs[f];
@@ -574,7 +582,6 @@ int write_tails(b200c_job* j, const std::vector<FileRec>& frs, const std::vector
   }
   // all tails with one scatter launch
   const size_t rec_bytes = sizeof(TailCopy) * nfiles;
-  CU(j->pin_small.reserve(rec_bytes));
   memcpy(j->pin_small.p, tcs.data(), rec_bytes);
   // the scatter kernel reads records and bytes straight from mapped pinned memory: no copy-engine queue involved
   launch_scatter_tails(reinterpret_cast<const TailCopy*>(j->pin_small.p), nfiles, j->pin_tails.p, j->out_buf.as<uint8_t>(), j->st);
@@ -763,6 +770,10 @@ int encode_stage(b200c_job* j, KeyCols mcols, uint64_t n_out, uint32_t min_s1, u
     W.idx_esz = j->idx_esz.as<uint32_t>();
     W.idx_eoff = j->idx_eoff.as<uint64_t>();
     W.idx_sep = j->idx_sep.as<KeyRec>();
+    // write_tails' pinned staging, reserved here: it runs while the emit kernel does, and a page-locked allocation would
+    // synchronise the device
+    CU(j->pin_tails.reserve((size_t)nfiles * 4096 + 64));
+    CU(j->pin_small.reserve(sizeof(TailCopy) * nfiles));
     // image layout: data blocks | index block (<= 45 B per data block + 9) | tail (properties, metaindex, footer)
     base_off.resize(nfiles + 1);
     uint64_t off = 0;
@@ -790,23 +801,30 @@ int encode_stage(b200c_job* j, KeyCols mcols, uint64_t n_out, uint32_t min_s1, u
     j->kt_begin("encode.blocklist");
     launch_encode_blocklist(mcols, ep, W, etiles, nblocks, err, st);
     j->kt_end();
-    // per-file statistics and the index blocks only need the block list: they run on the side stream while the main stream
-    // emits the data blocks (the index block of a file lies behind its data and filter blocks: disjoint bytes)
+    // The file tails (write_tails) need only the per-file records: statistics, boundary keys, index-block sizes.  Those kernels
+    // run on the main stream in front of the emit kernel (behind it they would wait for its last CTA, see
+    // launch_encode_emit); the records are gathered right behind them, and the host builds the tails while the data blocks are emitted.
+    j->kt_begin("encode.filestats+index_size");
+    launch_encode_index_size(mcols, ep, W, nblocks, j->sms, st, &j->launches);
+    launch_encode_filestats(mcols, W, nfiles, st);
+    j->kt_end();
+    if (int rc = gather_small(j, W.files)) return rc;
     CU(cudaEventRecord(j->evx[2], st));
-    CU(cudaStreamWaitEvent(j->st2, j->evx[2], 0));
-    {
-      const size_t slot = j->kt_begin("~encode.filestats+index", j->st2);
-      launch_encode_filestats(mcols, W, nfiles, j->st2);
-      launch_encode_index(mcols, ep, W, nblocks, nfiles, out_base_d, j->sms, j->st2, &j->launches);
-      j->kt_end(slot, j->st2);
-    }
-    CU(cudaEventRecord(j->evx[3], j->st2));
     uint64_t data_bytes = 0;
     for (uint32_t f = 0; f < nfiles; f++) data_bytes += frs[f].data_size;
     j->kt_begin("encode.emit");
     launch_encode_emit(mcols, ep, W, nblocks, out_base_d, data_bytes, err, j->sms, st);
     j->kt_end();
     j->launches += 3;
+    // The index blocks are written on the side stream beside the emit kernel (a file's index block lies behind its data and filter
+    // blocks: disjoint bytes).  They are enqueued after the emit so that the main stream does not idle while the host enqueues them.
+    CU(cudaStreamWaitEvent(j->st2, j->evx[2], 0));
+    {
+      const size_t slot = j->kt_begin("~encode.index", j->st2);
+      launch_encode_index_write(ep, W, nblocks, nfiles, out_base_d, j->sms, j->st2, &j->launches);
+      j->kt_end(slot, j->st2);
+    }
+    CU(cudaEventRecord(j->evx[3], j->st2));
     if (P.bloom_millibits_per_key) {
       j->kt_begin("encode.bloom_build");
       // scratch for the parallel part of the filter blocks' checksums: 8 u64 per full 1024-byte block
@@ -824,11 +842,23 @@ int encode_stage(b200c_job* j, KeyCols mcols, uint64_t n_out, uint32_t min_s1, u
       j->kt_end();
       j->launches += 3;
     }
+    // sync #3 waits for the records gathered in front of the emit kernel only.  The error word the emit, index and filter kernels
+    // may still raise is checked by finish_run().
+    CU(cudaEventSynchronize(j->evx[2]));
+    CU(cudaGetLastError());
+    take_small(j, h, W.files, &frs);
     CU(cudaStreamWaitEvent(st, j->evx[3], 0));
-    if (int rc = checked_sync(j, h, W.files, &frs)) return rc;  // sync #3: per-file records
-    if (frs.size() != nfiles) return fail(B200C_ERR_CUDA, "internal: output file count changed");
-    if (int rc = write_tails(j, frs, base_off)) return rc;
-    if (P.paranoid_file_checks) return paranoid_reread(j, mcols, frs, base_off);
+    int rc = map_dev_err((uint32_t)h[kSlotErr]);
+    if (rc == B200C_OK && frs.size() != nfiles) rc = fail(B200C_ERR_CUDA, "internal: output file count changed");
+    if (rc == B200C_OK) rc = write_tails(j, frs, base_off);
+    if (rc != B200C_OK) {  // the emit, filter and index kernels may still read the columns (caller-owned on the TableBuilder path)
+      cudaStreamSynchronize(st);  // (st waits for the side stream's index kernels)
+      return rc;
+    }
+    if (P.paranoid_file_checks) {
+      if (int rc = checked_sync(j, h)) return rc;  // an encoder error keeps its own status instead of the re-read's Corruption
+      return paranoid_reread(j, mcols, frs, base_off);
+    }
   }
   return B200C_OK;
 }
@@ -849,7 +879,10 @@ int finish_run(b200c_job* j) {
       CU(cudaMemcpyAsync(j->host_out.p + o.host_off, j->out_buf.as<uint8_t>() + o.dev_off, o.meta.file_size, cudaMemcpyDeviceToHost, st));
   }
   CU(cudaEventRecord(j->ev[4], st));
-  CU(cudaStreamSynchronize(st));
+  {  // the run's last checked synchronisation: errors the emit, index and filter kernels raised after sync #3
+    uint64_t h[kSmallSlots];
+    if (int rc = checked_sync(j, h)) return rc;
+  }
   float ms;
   cudaEventElapsedTime(&ms, j->ev[0], j->ev[1]);
   j->stats.decode_us = ms * 1000.0;

@@ -1135,9 +1135,15 @@ encode_blocklist_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t n, u
   }
 }
 
+// bytes of the index entries of the file whose data blocks are [b0, b0 + nb) (nb > 0): idx_eoff is the scan of idx_esz over all blocks
+__device__ __forceinline__ uint64_t index_entries_bytes(const EncodeWork& wk, uint64_t b0, uint64_t nb) {
+  return wk.idx_eoff[b0 + nb - 1] + wk.idx_esz[b0 + nb - 1] - wk.idx_eoff[b0];
+}
+
 // ------------------------------------------------------------------------------------------------ per-file statistics
 // One CTA per output file: stat tiles (merge tiles, or kEncTile entries on the TableBuilder-only path) that lie inside the file come
-// from their partial sums, the partly covered ones at its ends are read entry by entry; also the file's smallest / largest key.
+// from their partial sums, the partly covered ones at its ends are read entry by entry; also the file's smallest / largest key and
+// the size of its index block (the index entries' sizes and their scan are complete: launch_encode_index_size runs first).
 // Stat tile t covers the entries [prefix(t - 1), prefix(t)).
 __global__ void encode_filestats_kernel(KeyCols m, EncodeWork wk, uint32_t nfiles) {
   const uint32_t f = blockIdx.x;
@@ -1227,6 +1233,8 @@ __global__ void encode_filestats_kernel(KeyCols m, EncodeWork wk, uint32_t nfile
     wk.files[f].num_deletions = red[2];
     wk.files[f].smallest_seq = red[3];
     wk.files[f].largest_seq = red[4];
+    const uint64_t b0 = wk.files[f].first_block, nb = wk.files[f].n_blocks;
+    if (nb) wk.files[f].index_size = index_entries_bytes(wk, b0, nb) + 4 * nb + 4;  // entries | restart array | restart count
   }
 }
 
@@ -1960,8 +1968,7 @@ __global__ void encode_index_write_kernel(EncodeWork wk, uint64_t nblocks, uint3
     const KeyRec sep = wk.idx_sep[b];
     const uint32_t klen = sep.ulen + (fr.index_has_seq ? 8 : 0);
     const uint64_t eoff = wk.idx_eoff[b] - wk.idx_eoff[fr.first_block];
-    const uint64_t entries_bytes =
-        wk.idx_eoff[fr.first_block + fr.n_blocks - 1] + wk.idx_esz[fr.first_block + fr.n_blocks - 1] - wk.idx_eoff[fr.first_block];
+    const uint64_t entries_bytes = index_entries_bytes(wk, fr.first_block, fr.n_blocks);
     uint8_t* ib = out_base[br.file_idx] + fr.data_size + fr.filter_bytes;  // index block follows the last data block
     uint8_t* p = ib + eoff;
     uint8_t h[20];
@@ -1975,10 +1982,7 @@ __global__ void encode_index_write_kernel(EncodeWork wk, uint64_t nblocks, uint3
     // restart array: one restart per entry (index_block_restart_interval == 1)
     const uint64_t bi = b - fr.first_block;
     put_fixed32(ib + entries_bytes + 4 * bi, (uint32_t)eoff);
-    if (bi == 0) {
-      put_fixed32(ib + entries_bytes + 4 * fr.n_blocks, (uint32_t)fr.n_blocks);
-      wk.files[br.file_idx].index_size = entries_bytes + 4 * fr.n_blocks + 4;
-    }
+    if (bi == 0) put_fixed32(ib + entries_bytes + 4 * fr.n_blocks, (uint32_t)fr.n_blocks);
   }
 }
 // ---- checksum and trailer of a file's index block or filter block: both are one large block per file, behind its data blocks
@@ -2407,28 +2411,35 @@ void launch_encode_emit(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nbloc
   if (per_sm < 1) per_sm = 1;
   if (per_sm > ctas) per_sm = ctas;
   const uint64_t want = (nblocks + warps - 1) / warps;
-  // The persistent CTAs own every register of the SMs they sit on, so the side stream's kernels (per-file statistics, index
-  // blocks) queue behind the last emit CTA.
+  // The persistent CTAs own every register of the SMs they sit on, so the side stream's kernels (index-block writes and checksums)
+  // queue behind the last emit CTA.
   const uint64_t cap = (uint64_t)sms * per_sm;
   const unsigned grid = (unsigned)(want < cap ? want : cap);
   if (long_entries) encode_emit_long_kernel<<<grid, warps * 32, smem, st>>>(m, ep, w, nblocks, out_base, slot, err);
   else encode_emit_kernel<<<grid, warps * 32, smem, st>>>(m, ep, w, nblocks, out_base, slot, err);
 }
-void launch_encode_index(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nblocks, uint32_t nfiles, uint8_t* const* out_base,
-                         int sms, cudaStream_t st, uint64_t* launches) {
+static unsigned index_grid(uint64_t nblocks, int sms) {
+  const uint64_t g = (nblocks + 255) / 256;
+  return (unsigned)(g < (uint64_t)sms * 8 ? g : (uint64_t)sms * 8);
+}
+void launch_encode_index_size(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nblocks, int sms, cudaStream_t st, uint64_t* launches) {
   if (nblocks == 0) return;
-  unsigned g = (unsigned)((nblocks + 255) / 256);
-  if (g > (unsigned)sms * 8) g = (unsigned)sms * 8;
+  const unsigned g = index_grid(nblocks, sms);
   encode_index_sep_kernel<<<g, 256, 0, st>>>(m, w, nblocks);
   encode_index_size_kernel<<<g, 256, 0, st>>>(w, nblocks, ep.format_version);
   exclusive_scan<uint32_t>(w.idx_esz, w.idx_eoff, nblocks, w.scan_tmp, nullptr, st, launches);
-  encode_index_write_kernel<<<g, 256, 0, st>>>(w, nblocks, ep.format_version, out_base);
+  if (launches) *launches += 2;
+}
+void launch_encode_index_write(EncodeParams ep, EncodeWork w, uint64_t nblocks, uint32_t nfiles, uint8_t* const* out_base, int sms,
+                               cudaStream_t st, uint64_t* launches) {
+  if (nblocks == 0) return;
+  encode_index_write_kernel<<<index_grid(nblocks, sms), 256, 0, st>>>(w, nblocks, ep.format_version, out_base);
   if (ep.checksum == 4) {
     file_block_contrib_kernel<<<dim3(64, nfiles), 256, 0, st>>>(w.files, nfiles, kIndexBlock, out_base, w.idx_contrib, w.idx_contrib_off);
     if (launches) *launches += 1;
   }
   file_block_trailer_kernel<<<(nfiles + 3) / 4, 128, 0, st>>>(w.files, nfiles, kIndexBlock, ep.checksum, out_base, w.idx_contrib, w.idx_contrib_off);
-  if (launches) *launches += 4;
+  if (launches) *launches += 2;
 }
 void launch_block_checksums(uint32_t type, const uint8_t* data, const uint64_t* offsets, uint32_t n, uint8_t last_byte, uint32_t* out,
                             cudaStream_t st) {

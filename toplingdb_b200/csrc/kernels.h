@@ -239,13 +239,17 @@ void launch_encode_stitch(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nti
 void launch_encode_tilestate(KeyCols m, EncodeWork w, uint64_t ntiles, uint32_t hc, uint32_t* err, cudaStream_t st, uint64_t* launches);
 void launch_encode_blocklist(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t ntiles, uint64_t nblk_cap, uint32_t* err,
                              cudaStream_t st);
+// per-file statistics, boundary keys and index-block size: after launch_encode_index_size
 void launch_encode_filestats(KeyCols m, EncodeWork w, uint32_t nfiles, cudaStream_t st);
 uint32_t encode_emit_slice(uint32_t block_size);
 // out_base[f] = device address where file f's image starts; data_bytes = all data blocks incl. trailers (with m.n: selects the kernel)
 void launch_encode_emit(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nblocks, uint8_t* const* out_base, uint64_t data_bytes,
                         uint32_t* err, int sms, cudaStream_t st);
-void launch_encode_index(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nblocks, uint32_t nfiles, uint8_t* const* out_base,
-                         int sms, cudaStream_t st, uint64_t* launches);
+// index blocks in two steps: separators, entry sizes and their scan (what the file sizes need), then the entries, restart arrays and
+// trailers written into the images
+void launch_encode_index_size(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nblocks, int sms, cudaStream_t st, uint64_t* launches);
+void launch_encode_index_write(EncodeParams ep, EncodeWork w, uint64_t nblocks, uint32_t nfiles, uint8_t* const* out_base, int sms,
+                               cudaStream_t st, uint64_t* launches);
 void launch_block_checksums(uint32_t type, const uint8_t* data, const uint64_t* offsets, uint32_t n, uint8_t last_byte,
                             uint32_t* out, cudaStream_t st);
 
