@@ -42,6 +42,28 @@ def run_product(p, inputs, device_inputs=False, levels=None, **extra):
     return files, metas, st
 
 
+def _describe(ikey, value):
+    tr = struct.unpack("<Q", ikey[-8:])[0]
+    return f"user key {ikey[:-8].hex() or '(empty)'} seq {tr >> 8} type {tr & 0xff} value {len(value)} B"
+
+
+def assert_merged_matches(job, want, label=""):
+    """job: after run(until=2); want: [(internal key, value)] of the oracle's compaction iterator over the merged inputs.  Compares the
+    merge stage's output entry by entry and names the first one that differs (the input tile cannot be told from an output position;
+    the key is what leads to it)."""
+    recs = parse_key_recs(job.debug(T.native.DBG_MERGED_KEYS))
+    vals = job.debug(T.native.DBG_MERGED_VALUES)
+    off = 0
+    for i, ((uk, tr, vlen), (ik, v)) in enumerate(zip(recs, want)):
+        got_ik, got_v = uk + struct.pack("<Q", tr), vals[off:off + vlen]
+        assert got_ik == ik and got_v == v, \
+            f"{label}: merged entry {i} of {len(recs)} (oracle: {len(want)}) differs: device {_describe(got_ik, got_v)}, oracle {_describe(ik, v)}"
+        off += vlen
+    n = min(len(recs), len(want))
+    assert len(recs) == len(want), f"{label}: device wrote {len(recs)} merged entries, oracle {len(want)}; the first {n} agree" + \
+        ("" if n == 0 else f", the last of them {_describe(*want[n - 1])}")
+
+
 def parse_key_recs(b):
     """32-byte debug records -> list of (user_key bytes, trailer, vlen)"""
     out = []

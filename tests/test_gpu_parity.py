@@ -78,8 +78,7 @@ def _expected_merged(p, inputs):
 
 @pytest.mark.parametrize("case", [c for c in H.golden_cases() if c != "long_keys"])
 def test_merge_stage_matches_oracle(case):
-    from gpu_harness import job_from_params, parse_key_recs
-    T = _T()
+    from gpu_harness import assert_merged_matches, job_from_params
     g = H.load_golden(case)
     p = H.params_from_reference(g)
     want, _ = _expected_merged(p, g["inputs"])
@@ -87,14 +86,7 @@ def test_merge_stage_matches_oracle(case):
     for d in g["inputs"]:
         job.add_input(d)
     job.run(until=2)
-    recs = parse_key_recs(job.debug(T.native.DBG_MERGED_KEYS))
-    vals = job.debug(T.native.DBG_MERGED_VALUES)
-    assert len(recs) == len(want)
-    off = 0
-    for i, ((uk, tr, vlen), (ik, v)) in enumerate(zip(recs, want)):
-        assert uk + struct.pack("<Q", tr) == ik, i
-        assert vals[off:off + vlen] == v, i
-        off += vlen
+    assert_merged_matches(job, want, case)
     job.close()
 
 
