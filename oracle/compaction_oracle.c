@@ -376,7 +376,7 @@ static int index_cb(void* vctx, const uint8_t* key, size_t klen, const uint8_t* 
   idx_ctx* c = (idx_ctx*)vctx;
   uint64_t off = 0, size = 0, t = 0;
   const uint8_t* end = val + vlen;
-  if (shared == 0) {
+  if (shared == 0 || c->s->fv < 4) { /* before format_version 4 every index value is a whole BlockHandle */
     val = get_varint(val, end, &off);
     get_varint(val, end, &size);
   } else {

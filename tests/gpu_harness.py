@@ -64,6 +64,29 @@ def assert_merged_matches(job, want, label=""):
         ("" if n == 0 else f", the last of them {_describe(*want[n - 1])}")
 
 
+def assert_decoded_matches(job, run, entries, label="", where=None):
+    """job: after run(until=1); entries: [(internal key, value)] that run `run` must hold, in order; where: for every entry a dict
+    (block, offset, phase, path) -- the block index in the file, the entry's offset in the block, the block's file offset mod 16 and
+    the path the decoder is expected to take (decode_cases.located_entries).  Names the first entry that differs."""
+    recs = parse_key_recs(job.debug(T.native.DBG_DECODED_KEYS, run))
+    vals = job.debug(T.native.DBG_DECODED_VALUES, run)
+    off = 0
+
+    def at(i):
+        if where is None or i >= len(where):
+            return ""
+        w = where[i]
+        return f" (block {w['block']}, offset {w['offset']} in the block, phase {w['phase']}, expected path {w['path']})"
+    for i, ((uk, tr, vlen), (ik, v)) in enumerate(zip(recs, entries)):
+        got_ik, got_v = uk + struct.pack("<Q", tr), vals[off:off + vlen]
+        assert got_ik == ik and got_v == v, \
+            f"{label}: run {run} entry {i}{at(i)} differs: device {_describe(got_ik, got_v)}, table {_describe(ik, v)}"
+        off += vlen
+    n = min(len(recs), len(entries))
+    assert len(recs) == len(entries), f"{label}: run {run} decoded {len(recs)} entries, the table holds {len(entries)}; the first {n} agree" + \
+        ("" if n == len(entries) else f"; the next one is{at(n)}")
+
+
 def parse_key_recs(b):
     """32-byte debug records -> list of (user_key bytes, trailer, vlen)"""
     out = []

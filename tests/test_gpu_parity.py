@@ -44,8 +44,8 @@ def test_device_block_checksums_match_oracle():
 
 @pytest.mark.parametrize("case", [c for c in H.golden_cases() if c != "long_keys"])
 def test_decode_stage_matches_oracle(case):
-    from gpu_harness import job_from_params, parse_key_recs
-    T = _T()
+    from decode_cases import located_entries
+    from gpu_harness import assert_decoded_matches, job_from_params
     g = H.load_golden(case)
     p = H.params_from_reference(g)
     job = job_from_params(p)
@@ -53,15 +53,9 @@ def test_decode_stage_matches_oracle(case):
         job.add_input(d)
     job.run(until=1)
     for r, data in enumerate(g["inputs"]):
-        want = sstfmt.parse_sst(data)["entries"]
-        recs = parse_key_recs(job.debug(T.native.DBG_DECODED_KEYS, r))
-        vals = job.debug(T.native.DBG_DECODED_VALUES, r)
-        assert len(recs) == len(want)
-        off = 0
-        for (uk, tr, vlen), (ik, v) in zip(recs, want):
-            assert uk + struct.pack("<Q", tr) == ik
-            assert vals[off:off + vlen] == v
-            off += vlen
+        want, where = located_entries(data)
+        assert want == sstfmt.parse_sst(data)["entries"]
+        assert_decoded_matches(job, r, want, case, where)
     job.close()
 
 
