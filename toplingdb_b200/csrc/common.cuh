@@ -146,6 +146,110 @@ __device__ __forceinline__ bool ikey_less(const Key& a, const Key& b) {
   if (c) return c < 0;
   return a.tr > b.tr;  // larger (seq,type) first
 }
+__device__ __forceinline__ bool same_ukey(const Key& a, uint64_t hi, uint64_t lo, uint32_t ulen) {
+  return (a.hi == hi) & (a.lo == lo) & (a.ulen == ulen);
+}
+__device__ __forceinline__ bool same_ukey(const Key& a, const Key& b) { return same_ukey(a, b.hi, b.lo, b.ulen); }
+// first entry of [a, b) of sorted key columns whose user key is >= (hi, lo, ulen), or > it when `upper`
+__device__ __forceinline__ uint64_t ukey_bound(const KeyCols& c, uint64_t a, uint64_t b, uint64_t hi, uint64_t lo, uint32_t ulen, bool upper) {
+  while (a < b) {
+    const uint64_t mid = a + ((b - a) >> 1);
+    const ulonglong2 p = c.pfx[mid];
+    const int d = ukey_cmp(p.x, p.y, meta_ulen(c.meta[mid]), hi, lo, ulen);
+    if (d < 0 || (upper && d == 0)) a = mid + 1;
+    else b = mid;
+  }
+  return a;
+}
+
+// ---- decoupled look-back: exclusive prefix sums over parts (decoded blocks, merge tiles) that finish in any order -----------
+// One state word per part, zero until the part publishes: the top two bits are the flag (kLbCount: the part's own count,
+// kLbPrefix: the inclusive prefix through the part), the low 62 bits are the value.
+constexpr unsigned long long kLbCount = 1ull << 62, kLbPrefix = 2ull << 62, kLbValue = (1ull << 62) - 1;
+// value of a state word (also of a plain prefix without flag bits, as encode_sizes_kernel writes them)
+__device__ __forceinline__ uint64_t lb_value(unsigned long long sv) { return sv & kLbValue; }
+// part p's own count; part 0's count is already its inclusive prefix.  One thread per part.
+__device__ __forceinline__ void lb_publish(unsigned long long* state, uint64_t p, uint64_t cnt) {
+  atomicExch(&state[p], (p == 0 ? kLbPrefix : kLbCount) | cnt);
+}
+// One warp, after part p published its count: the sum of the counts of the parts in front of p, which then becomes p's inclusive
+// prefix.  Lanes read 32 predecessors per step and stop at the nearest inclusive prefix; a predecessor that has not published yet
+// is polled every sleep_ns nanoseconds, which leaves the issue slots to warps that still work.  Every lane returns the sum.
+__device__ __forceinline__ uint64_t lb_exclusive_prefix(unsigned long long* state, uint64_t p, uint64_t cnt, unsigned lane, uint32_t sleep_ns) {
+  uint64_t base = 0;
+  if (p != 0) {
+    int64_t look = (int64_t)p - 1;
+    while (true) {
+      const int64_t idx = look - lane;
+      unsigned long long sv = kLbPrefix;  // virtual parts before 0 contribute a zero prefix
+      if (idx >= 0) {
+        sv = *((volatile unsigned long long*)&state[idx]);
+        while ((sv >> 62) == 0) {
+          __nanosleep(sleep_ns);
+          sv = *((volatile unsigned long long*)&state[idx]);
+        }
+      }
+      const unsigned pre_mask = __ballot_sync(0xffffffffu, (sv >> 62) == 2);
+      const int first_pre = pre_mask ? __ffs(pre_mask) - 1 : 32;
+      uint64_t contrib = ((int)lane <= first_pre) ? lb_value(sv) : 0;
+#pragma unroll
+      for (int dd = 16; dd; dd >>= 1) contrib += __shfl_xor_sync(0xffffffffu, contrib, dd);
+      base += contrib;
+      if (pre_mask) break;
+      look -= 32;
+    }
+    if (lane == 0) atomicExch(&state[p], kLbPrefix | (base + cnt));
+  }
+  return base;
+}
+
+// ---- partial sums of a TileStat (kernels.h): key bytes, value bytes, deletions, smallest / largest sequence number ---------------
+// Each thread adds entries (or whole stat tiles), then flush() reduces over the warp and adds into five shared slots that
+// stat_slots_init prepared.  C is the width of the key-byte and deletion sums: 32 bits where a thread holds few entries, so that
+// each is reduced by one redux instruction.
+__device__ __forceinline__ void stat_slots_init(unsigned long long* slots, uint32_t t) {
+  if (t < 5) slots[t] = t == 3 ? ~0ull : 0ull;
+}
+template <typename C>
+struct StatAcc {
+  C kb = 0, nd = 0;
+  unsigned long long vb = 0, smin = ~0ull, smax = 0;
+  __device__ __forceinline__ void add(C key_bytes, unsigned long long value_bytes, C deletions, unsigned long long seq_lo,
+                                      unsigned long long seq_hi) {
+    kb += key_bytes;
+    vb += value_bytes;
+    nd += deletions;
+    smin = seq_lo < smin ? seq_lo : smin;
+    smax = seq_hi > smax ? seq_hi : smax;
+  }
+  __device__ __forceinline__ void add_entry(uint32_t key_bytes, uint32_t vlen, uint64_t tr) {
+    add(key_bytes, vlen, is_deletion_type((uint32_t)(tr & 0xff)), tr >> 8, tr >> 8);
+  }
+  __device__ __forceinline__ void flush(unsigned long long* slots) {
+    if constexpr (sizeof(C) == 4) {
+      kb = __reduce_add_sync(0xffffffffu, kb);
+      nd = __reduce_add_sync(0xffffffffu, nd);
+    }
+#pragma unroll
+    for (int d = 16; d; d >>= 1) {
+      if constexpr (sizeof(C) == 8) {
+        kb += __shfl_xor_sync(0xffffffffu, kb, d);
+        nd += __shfl_xor_sync(0xffffffffu, nd, d);
+      }
+      vb += __shfl_xor_sync(0xffffffffu, vb, d);
+      const unsigned long long a = __shfl_xor_sync(0xffffffffu, smin, d), b = __shfl_xor_sync(0xffffffffu, smax, d);
+      smin = a < smin ? a : smin;
+      smax = b > smax ? b : smax;
+    }
+    if ((threadIdx.x & 31) == 0) {
+      atomicAdd(&slots[0], (unsigned long long)kb);
+      atomicAdd(&slots[1], vb);
+      atomicAdd(&slots[2], (unsigned long long)nd);
+      atomicMin(&slots[3], smin);
+      atomicMax(&slots[4], smax);
+    }
+  }
+};
 
 // ---- XXH3-64, seed 0, default secret ------------------------------------------------------------------------
 static __device__ __constant__ uint8_t kXxhSecret[192] = {

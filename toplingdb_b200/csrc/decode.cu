@@ -393,39 +393,7 @@ __device__ __noinline__ uint32_t decode_interval_seq(const uint8_t* p, const uin
   return n;
 }
 
-// global position of block b: decoupled look-back over the per-block states (flag in the two top bits: 1 = this block's
-// count, 2 = inclusive prefix).  The block's own count must already be published.
-__device__ __forceinline__ uint64_t block_lookback(unsigned long long* blk_state, uint32_t b, uint32_t cnt, unsigned lane) {
-  const unsigned long long kPre = 2ull << 62, kVal = (1ull << 62) - 1;
-  uint64_t base = 0;
-  if (b != 0) {
-    int64_t look = (int64_t)b - 1;
-    while (true) {
-      const int64_t idx = look - lane;
-      unsigned long long sv = kPre;  // virtual blocks before 0 contribute a zero prefix
-      if (idx >= 0) {
-        sv = *((volatile unsigned long long*)&blk_state[idx]);
-        while ((sv >> 62) == 0) {
-          __nanosleep(40);  // the predecessor is still walking its block: leave the issue slots to working warps
-          sv = *((volatile unsigned long long*)&blk_state[idx]);
-        }
-      }
-      const unsigned pre_mask = __ballot_sync(0xffffffffu, (sv >> 62) == 2);
-      const int first_pre = pre_mask ? __ffs(pre_mask) - 1 : 32;
-      uint64_t contrib = ((int)lane <= first_pre) ? (sv & kVal) : 0;
-#pragma unroll
-      for (int dd = 16; dd; dd >>= 1) contrib += __shfl_xor_sync(0xffffffffu, contrib, dd);
-      base += contrib;
-      if (pre_mask) break;
-      look -= 32;
-    }
-    if (lane == 0) atomicExch(&blk_state[b], kPre | (base + cnt));
-  }
-  return base;
-}
-__device__ __forceinline__ void publish_block_count(unsigned long long* blk_state, uint32_t b, uint32_t cnt, unsigned lane) {
-  if (lane == 0) atomicExch(&blk_state[b], ((b == 0 ? 2ull : 1ull) << 62) | cnt);
-}
+constexpr uint32_t kLookbackSleepNs = 40;  // look-back poll period: a block that has not published its count is still being walked
 __device__ __forceinline__ void record_run_starts(const FileDesc* __restrict__ files, int nfiles, int f, uint32_t b, uint32_t nblk, uint64_t base,
                                                   uint32_t cnt, uint64_t* __restrict__ run_start, uint64_t* __restrict__ total_out) {
   // runs start where their first block starts (runs without blocks start where the next one does)
@@ -559,7 +527,7 @@ __device__ __forceinline__ bool decode_block_fast(DecWarpSmem& ws, uint32_t sp, 
   const uint32_t inc = warp_incl_scan(c);
   const uint32_t cnt = __shfl_sync(0xffffffffu, inc, 31);
   if (lane <= nr) sts16(sex + 2 * lane, inc - c);  // ex[nr] = cnt
-  publish_block_count(blk_state, b, cnt, lane);    // successors can look back while this warp checksums
+  if (lane == 0) lb_publish(blk_state, b, cnt);  // successors can look back while this warp checksums
   {
     const uint32_t ctype = lds8(sp + size);
     if (ctype != 0) {
@@ -574,7 +542,7 @@ __device__ __forceinline__ bool decode_block_fast(DecWarpSmem& ws, uint32_t sp, 
       }
     }
   }
-  const uint64_t base = block_lookback(blk_state, b, cnt, lane);
+  const uint64_t base = lb_exclusive_prefix(blk_state, b, cnt, lane, kLookbackSleepNs);
   if (lane == 0) record_run_starts(files, nfiles, f, b, nblk, base, cnt, run_start, total_out);
   if (!ok || cnt == 0) return true;
   if (base + cnt > n_total) {
@@ -719,8 +687,8 @@ __device__ __noinline__ void decode_block_slow(const uint8_t* p, uint32_t size, 
     }
   }
   if (!ok) cnt = 0;  // a rejected block contributes no entries (the job fails anyway)
-  publish_block_count(blk_state, b, cnt, lane);
-  const uint64_t base = block_lookback(blk_state, b, cnt, lane);
+  if (lane == 0) lb_publish(blk_state, b, cnt);
+  const uint64_t base = lb_exclusive_prefix(blk_state, b, cnt, lane, kLookbackSleepNs);
   if (lane == 0) record_run_starts(files, nfiles, f, b, nblk, base, cnt, run_start, total_out);
   if (!ok || cnt == 0) return;
   if (base + cnt > n_total) {
@@ -773,11 +741,11 @@ block_decode_fused_kernel(const FileDesc* __restrict__ files, int nfiles, const 
     const uint8_t* src = inflated ? arena + (bo & (kBlkArenaBit - 1)) : files[f].base + (bo & kBlkOffMask);
     const uint32_t size = blk_size[b], cksum = inflated ? 0u : files[f].cksum;
     if (size == 0) {  // outside the sub-compaction's key range (index_decode_kernel): an empty block, nothing is read
-      publish_block_count(blk_state, b, 0, lane);
+      if (lane == 0) lb_publish(blk_state, b, 0);
       // its position only matters where a run starts / the stream ends; every 32nd skipped block still resolves its prefix so that
       // the look-back of the next real block does not have to walk a whole skipped stretch
       if (files[f].gblk_first == b || b + 1 == nblk || (b & 31u) == 31u) {
-        const uint64_t base0 = block_lookback(blk_state, b, 0, lane);
+        const uint64_t base0 = lb_exclusive_prefix(blk_state, b, 0, lane, kLookbackSleepNs);
         if (lane == 0) record_run_starts(files, nfiles, f, b, nblk, base0, 0, run_start, total_out);
       }
       continue;

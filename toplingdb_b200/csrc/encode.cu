@@ -50,10 +50,10 @@ encode_sizes_kernel(KeyCols m, const unsigned long long* __restrict__ n_dev, uin
     s_mx = 0;
   }
   for (uint64_t tile = blockIdx.x; tile < ntiles; tile += gridDim.x) {
-    if (threadIdx.x < 5) red[threadIdx.x] = threadIdx.x == 3 ? ~0ull : 0ull;
+    stat_slots_init(red, threadIdx.x);
     __syncthreads();
     const uint64_t t0 = tile * kEncTile, t1 = (t0 + kEncTile) < n ? (t0 + kEncTile) : n;
-    unsigned long long kb = 0, vb = 0, nd = 0, smin = ~0ull, smax = 0;
+    StatAcc<unsigned long long> st;
     // four entries per thread in flight; the previous entry (for the shared-prefix length) comes from the neighbouring lane,
     // only lane 0 of a warp fetches it from memory
     constexpr int kB = 4;
@@ -99,31 +99,11 @@ encode_sizes_kernel(KeyCols m, const unsigned long long* __restrict__ n_dev, uin
           eshared[i] = (uint8_t)sh;
           mn = s1 < mn ? s1 : mn;
           mxs = s1 > mxs ? s1 : mxs;
-          kb += ks;
-          vb += vs;
-          nd += is_deletion_type((uint32_t)(ctr[q] & 0xff));
-          const uint64_t sq = ctr[q] >> 8;
-          smin = sq < smin ? sq : smin;
-          smax = sq > smax ? sq : smax;
+          st.add_entry(ks, vs, ctr[q]);
         }
       }
     }
-#pragma unroll
-    for (int d = 16; d; d >>= 1) {
-      kb += __shfl_xor_sync(0xffffffffu, kb, d);
-      vb += __shfl_xor_sync(0xffffffffu, vb, d);
-      nd += __shfl_xor_sync(0xffffffffu, nd, d);
-      const unsigned long long a = __shfl_xor_sync(0xffffffffu, smin, d), b = __shfl_xor_sync(0xffffffffu, smax, d);
-      smin = a < smin ? a : smin;
-      smax = b > smax ? b : smax;
-    }
-    if ((threadIdx.x & 31) == 0) {
-      atomicAdd(&red[0], kb);
-      atomicAdd(&red[1], vb);
-      atomicAdd(&red[2], nd);
-      atomicMin(&red[3], smin);
-      atomicMax(&red[4], smax);
-    }
+    st.flush(red);
     __syncthreads();
     if (threadIdx.x == 0) {
       tstat[tile] = TileStat{red[0], red[1], red[2], red[3], red[4]};
@@ -1150,12 +1130,11 @@ __global__ void encode_filestats_kernel(KeyCols m, EncodeWork wk, uint32_t nfile
   if (f >= nfiles) return;
   const uint64_t f0 = wk.files[f].first_entry, f1 = f0 + wk.files[f].n_entries;
   __shared__ unsigned long long red[5];
-  if (threadIdx.x < 5) red[threadIdx.x] = threadIdx.x == 3 ? ~0ull : 0ull;
+  stat_slots_init(red, threadIdx.x);
   __syncthreads();
-  const unsigned long long kVal = (1ull << 62) - 1;
-  unsigned long long kb = 0, vb = 0, nd = 0, smin = ~0ull, smax = 0;
+  StatAcc<unsigned long long> st;
   if (f1 > f0) {
-    auto tile_start = [&](uint64_t t) -> uint64_t { return t ? (wk.tprefix[t - 1] & kVal) : 0; };
+    auto tile_start = [&](uint64_t t) -> uint64_t { return t ? lb_value(wk.tprefix[t - 1]) : 0; };
     auto first_tile_starting_at_or_after = [&](uint64_t e) -> uint64_t {  // tile starts are non-decreasing
       uint64_t lo = 0, hi = wk.nstat;
       while (lo < hi) {
@@ -1171,35 +1150,25 @@ __global__ void encode_filestats_kernel(KeyCols m, EncodeWork wk, uint32_t nfile
       uint64_t lo = 0, hi = wk.nstat;
       while (lo < hi) {
         const uint64_t mid = lo + ((hi - lo) >> 1);
-        if ((wk.tprefix[mid] & kVal) <= f1) lo = mid + 1;
+        if (lb_value(wk.tprefix[mid]) <= f1) lo = mid + 1;
         else hi = mid;
       }
       tB = lo;
     }
     auto scan_entries = [&](uint64_t lo, uint64_t hi) {
       for (uint64_t i = lo + threadIdx.x; i < hi; i += blockDim.x) {
-        const uint64_t tr = m.tr[i];
         const uint32_t mt = m.meta[i];
-        kb += meta_ulen(mt) + 8;
-        vb += meta_vlen(mt);
-        nd += is_deletion_type((uint32_t)(tr & 0xff));
-        const uint64_t sq = tr >> 8;
-        smin = sq < smin ? sq : smin;
-        smax = sq > smax ? sq : smax;
+        st.add_entry(meta_ulen(mt) + 8, meta_vlen(mt), m.tr[i]);
       }
     };
     if (tA >= tB) {
       scan_entries(f0, f1);  // the file covers no whole stat tile
     } else {
       scan_entries(f0, tile_start(tA));
-      scan_entries(wk.tprefix[tB - 1] & kVal, f1);
+      scan_entries(lb_value(wk.tprefix[tB - 1]), f1);
       for (uint64_t t = tA + threadIdx.x; t < tB; t += blockDim.x) {
         const TileStat ts = wk.tstat[t];
-        kb += ts.raw_key;
-        vb += ts.raw_value;
-        nd += ts.deletions;
-        smin = ts.smallest_seq < smin ? ts.smallest_seq : smin;
-        smax = ts.largest_seq > smax ? ts.largest_seq : smax;
+        st.add(ts.raw_key, ts.raw_value, ts.deletions, ts.smallest_seq, ts.largest_seq);
       }
     }
     if (threadIdx.x < 2) {  // boundary keys
@@ -1210,22 +1179,7 @@ __global__ void encode_filestats_kernel(KeyCols m, EncodeWork wk, uint32_t nfile
       else wk.files[f].largest = kr;
     }
   }
-#pragma unroll
-  for (int d = 16; d; d >>= 1) {
-    kb += __shfl_xor_sync(0xffffffffu, kb, d);
-    vb += __shfl_xor_sync(0xffffffffu, vb, d);
-    nd += __shfl_xor_sync(0xffffffffu, nd, d);
-    const unsigned long long a = __shfl_xor_sync(0xffffffffu, smin, d), b = __shfl_xor_sync(0xffffffffu, smax, d);
-    smin = a < smin ? a : smin;
-    smax = b > smax ? b : smax;
-  }
-  if ((threadIdx.x & 31) == 0) {
-    atomicAdd(&red[0], kb);
-    atomicAdd(&red[1], vb);
-    atomicAdd(&red[2], nd);
-    atomicMin(&red[3], smin);
-    atomicMax(&red[4], smax);
-  }
+  st.flush(red);
   __syncthreads();
   if (threadIdx.x == 0) {
     wk.files[f].raw_key_size = red[0];
@@ -2261,17 +2215,7 @@ __global__ void gp_rank_kernel(KeyCols m, const GpKey* __restrict__ smallest, co
                                uint64_t* __restrict__ lo, uint64_t* __restrict__ eq, uint64_t* __restrict__ hi) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  auto bound = [&](const GpKey& k, bool upper) -> uint64_t {  // first entry with user key >= k (upper: > k)
-    uint64_t a = 0, b = m.n;
-    while (a < b) {
-      const uint64_t mid = a + ((b - a) >> 1);
-      const ulonglong2 p = m.pfx[mid];
-      const int c = ukey_cmp(p.x, p.y, meta_ulen(m.meta[mid]), k.hi, k.lo, k.ulen);
-      if (c < 0 || (upper && c == 0)) a = mid + 1;
-      else b = mid;
-    }
-    return a;
-  };
+  auto bound = [&](const GpKey& k, bool upper) -> uint64_t { return ukey_bound(m, 0, m.n, k.hi, k.lo, k.ulen, upper); };
   lo[i] = bound(smallest[i], false);
   eq[i] = bound(largest[i], false);
   hi[i] = bound(largest[i], true);
