@@ -1,7 +1,7 @@
 // tests/native/gp_rules_sim.cc — test infrastructure: runs the product's grandparent cut rules (toplingdb_b200/csrc/gp_rules.h, the
-// same code the encoder's stitch kernel runs on the device) on the CPU over the block layout of a finished job, the way
-// encode.cu's chase_tile drives them, and reports where they cut.  tests/test_gp_rules_host.py compares that with the file
-// boundaries the oracle / the reference produced.
+// same code the encoder's stitch kernel runs on the device) on the CPU over the block layout of a finished job through the two
+// steps encode.cu's chase_tile takes (gp_block_cut per open block, gp_size_cut behind a size cut), and reports where they cut.
+// tests/test_gp_rules_host.py compares that with the file boundaries the oracle / the reference produced.
 #include <stdint.h>
 
 #include "gp_rules.h"
@@ -25,31 +25,19 @@ int64_t gp_rules_sim(uint32_t n_gp, const uint64_t* lo, const uint64_t* eq, cons
   uint64_t ncuts = 0;
   for (uint64_t b = 0; b < n_blocks; b++) {
     const uint64_t a = blk_first[b], end = a + blk_count[b], foff = blk_foff[b];
-    if (last_of_file[b] && foff >= max_output_file_size) {
-      // the size rule closed the file behind this single-entry block: ShouldStopBefore(end) moved the boundary state first
+    if (last_of_file[b] && foff >= max_output_file_size) {  // the size rule closed the file behind this single-entry block
       if (blk_count[b] != 1) return -(int64_t)(b + 1);
-      if (end < n_entries) {
-        gp_advance(g, c, end);
-        gp_file_started(g, c, end);
-      }
+      gp_size_cut(g, c, end, n_entries);
       continue;
     }
-    // entries a < e <= end are added while this block is open and see `foff` flushed bytes
-    bool cut = false;
-    uint64_t ev;
-    while ((ev = gp_next_event(g, c)) <= end && ev < n_entries) {
-      const uint64_t prev = g.overlapped;
-      const uint32_t crossed = gp_advance(g, c, ev);
-      if (gp_should_stop(g, c, crossed, prev, foff)) {
-        if (ev != end || !last_of_file[b]) return -(int64_t)(b + 1);  // the layout does not end a file here
-        if (ncuts < cap) cuts[ncuts] = ev;
-        ncuts++;
-        gp_file_started(g, c, ev);
-        cut = true;
-        break;
-      }
+    const uint64_t cut = gp_block_cut(g, c, end, n_entries, foff);
+    if (cut != ~0ull) {
+      if (cut != end || !last_of_file[b]) return -(int64_t)(b + 1);  // the layout does not end a file here
+      if (ncuts < cap) cuts[ncuts] = cut;
+      ncuts++;
+    } else if (last_of_file[b] && end < n_entries) {
+      return -(int64_t)(b + 1);  // the layout ends a file the rules would not end
     }
-    if (!cut && last_of_file[b] && end < n_entries) return -(int64_t)(b + 1);  // the layout ends a file the rules would not end
   }
   return (int64_t)ncuts;
 }

@@ -738,7 +738,7 @@ int encode_stage(b200c_job* j, KeyCols mcols, uint64_t n_out, uint32_t min_s1, u
       j->kt_end(slot, j->st2);
     }
     j->kt_begin("encode.tables");
-    launch_encode_tables(mcols, ep, W, etiles, hc, max_s1, err, st);
+    launch_encode_tables(mcols, ep, W, etiles, hc, max_s1, st);
     j->kt_end();
     {
       const size_t slot = j->kt_begin("~encode.stitch_retry", j->st2);

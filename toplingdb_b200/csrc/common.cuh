@@ -753,6 +753,10 @@ __device__ __forceinline__ uint32_t shared_prefix(uint64_t ahi, uint64_t alo, ui
 __device__ __forceinline__ uint32_t entry_size(uint32_t shared, uint32_t ks, uint32_t vs) {
   return varint_len32(shared) + varint_len32(ks - shared) + varint_len32(vs) + (ks - shared) + vs;
 }
+// restart surcharge: entry_size of the entry stored as a restart entry (shared == 0) minus entry_size with `shared` bytes shared
+__host__ __device__ __forceinline__ uint32_t restart_surcharge(uint32_t shared, uint32_t ks) {
+  return 1u + varint_len32(ks) + shared - varint_len32(shared) - varint_len32(ks - shared);
+}
 // ---- warp scans ---------------------------------------------------------------------------------------------
 // Cooperative global -> shared copy with kDepth loads per thread in flight: a plain `dst[i] = src[i]` loop issues in
 // order, so each iteration would wait for its own DRAM round trip before the next load leaves.

@@ -166,9 +166,7 @@ __device__ void build_window(Window<PT>& w, const KeyCols& m, const uint32_t* es
     for (int i = 0; i < kBatch; i++) {
       const uint32_t j = jb + i * kEncThreads + threadIdx.x;
       if (j < wlen) {
-        const uint32_t sh = shv[i], ks = meta_ulen(mtv[i]) + 8;
-        // D = s0 - s1 with s0 = encoded size when shared == 0
-        const uint32_t d = 1u + varint_len32(ks) + sh - varint_len32(sh) - varint_len32(ks - sh);
+        const uint32_t d = restart_surcharge(shv[i], meta_ulen(mtv[i]) + 8);
         w.Q[j] = d;
         w.P[j + 1] = (PT)s1v[i];
         mx = s1v[i] + d > mx ? s1v[i] + d : mx;
@@ -399,35 +397,63 @@ __device__ __forceinline__ TileRow ldcg_row(const TileRow* p) {
   return r;
 }
 static_assert(sizeof(TileRow) == 16, "TileRow is moved as one 16-byte vector");
+
+// ---- the row walk: a chain position (entry, blocks, bytes) crosses a span (tile or group) by the span's row of its entry point
+// r = row of entry point cc of a span whose rows start at `rows`; false when cc is not tabulated (cc >= hc, or the chain from cc
+// leaves the window).  kL2: the rows are written by other CTAs of the running tables kernel
+template <bool kL2 = false>
+__device__ __forceinline__ bool tabulated_row(const TileRow* rows, uint64_t cc, uint32_t hc, TileRow& r) {
+  if (cc >= hc) return false;
+  r = kL2 ? ldcg_row(rows + cc) : rows[cc];
+  return r.exit != 0xffffffffu;
+}
+// moves the chain position past the span starting at entry `start` by its row r
+__device__ __forceinline__ void follow_row(const TileRow& r, uint64_t start, uint64_t& a, uint64_t& blk, uint64_t& bytes) {
+  a = start + r.exit;
+  blk += r.nblk;
+  bytes += r.bytes;
+}
+// the row of entry point x of a tile whose nxt / disk sit in shared memory: follows nxt to the first block start behind the tile's
+// tl entries (exit 0xffffffff: a block does not end inside the window).  mark != nullptr: flags every block start on the way
+__device__ __forceinline__ TileRow follow_nxt(const uint16_t* nxt, const uint32_t* disk, uint32_t x, uint32_t tl, uint8_t* mark = nullptr) {
+  TileRow r{0, 0, 0};
+  while (x < tl) {
+    const uint32_t y = nxt[x];
+    if (y == 0xffff || y <= x) {
+      r.exit = 0xffffffffu;
+      return r;
+    }
+    if (mark) mark[x] = 1;
+    r.bytes += disk[x];
+    r.nblk++;
+    x = y;
+  }
+  r.exit = x;
+  return r;
+}
+// The one descend rule of the stitch walk and the block list: a span cannot be crossed by its row r (from the chain position
+// whose file holds `foff` bytes) when the row is not tabulated, the size rule fires inside, the stream ends inside, or a grandparent
+// boundary (next_ev: the next event of the rules, or in the block list the next recorded cut) lies inside.
+__device__ __forceinline__ bool must_descend(bool tabulated, const TileRow& r, uint64_t start, uint64_t n, uint64_t foff,
+                                             const EncodeParams& ep, uint64_t next_ev) {
+  return !tabulated || (ep.output_level != 0 && foff + r.bytes >= ep.max_output_file_size) || start + r.exit >= n ||
+         next_ev <= start + r.exit;
+}
+
 // composes the transfer functions of the tiles [t0, t1) of group g per entry-point candidate (all threads of the CTA)
 __device__ void compose_group(const EncodeWork& wk, uint64_t n, uint64_t g, uint64_t t0, uint64_t t1, uint32_t hc) {
   const uint64_t gstart = t0 * (uint64_t)kTT;
   for (uint32_t c = threadIdx.x; c < hc; c += blockDim.x) {
-    uint64_t x = gstart + c, bytes = 0;
-    uint32_t nb = 0;
-    bool bad = false;
+    uint64_t x = gstart + c, blk = 0, bytes = 0;
+    bool ok = true;
     for (uint64_t t = t0; t < t1 && x < n; t++) {
       const uint64_t tstart = t * (uint64_t)kTT, tend = (tstart + kTT) < n ? (tstart + kTT) : n;
       if (x >= tend) continue;  // no block starts in this tile
-      const uint64_t cc = x - tstart;
-      if (cc >= hc) {
-        bad = true;
-        break;
-      }
-      const TileRow r = ldcg_row(&wk.rows[t * hc + cc]);
-      if (r.exit == 0xffffffffu) {
-        bad = true;
-        break;
-      }
-      x = tstart + r.exit;
-      nb += r.nblk;
-      bytes += r.bytes;
+      TileRow r;
+      if (!(ok = tabulated_row<true>(wk.rows + t * hc, x - tstart, hc, r))) break;
+      follow_row(r, tstart, x, blk, bytes);
     }
-    TileRow o;
-    o.exit = bad ? 0xffffffffu : (uint32_t)(x - gstart);  // relative to the group start
-    o.nblk = nb;
-    o.bytes = bytes;
-    wk.grows[g * hc + c] = o;
+    wk.grows[g * hc + c] = TileRow{ok ? (uint32_t)(x - gstart) : 0xffffffffu, (uint32_t)blk, bytes};  // exit relative to the group
   }
 }
 
@@ -440,8 +466,7 @@ struct TablesSmem {
 };
 template <typename PT>
 __global__ void __launch_bounds__(kEncThreads, sizeof(PT) == 4 ? 3 : 2)
-encode_tables_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t n, uint32_t hc, uint16_t* __restrict__ g_nxt,
-                     uint32_t* __restrict__ g_disk, uint32_t* __restrict__ err) {
+encode_tables_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t n, uint32_t hc) {
   extern __shared__ __align__(16) uint8_t smem_raw[];
   TablesSmem<PT>& s = *reinterpret_cast<TablesSmem<PT>*>(smem_raw);
   const uint64_t tile = blockIdx.x, wstart = tile * (uint64_t)kTT;
@@ -481,31 +506,12 @@ encode_tables_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t n, uint
   }
   __syncthreads();
   for (uint32_t j = threadIdx.x; j < tl; j += kEncThreads) {  // coalesced copy for the block-list pass
-    g_nxt[wstart + j] = s.nxt[j];
-    g_disk[wstart + j] = s.disk[j];
+    wk.nxt[wstart + j] = s.nxt[j];
+    wk.disk[wstart + j] = s.disk[j];
   }
   __syncthreads();
-  for (uint32_t c = threadIdx.x; c < hc; c += kEncThreads) {
-    uint32_t x = c, nb = 0;
-    uint64_t bytes = 0;
-    bool bad = false;
-    while (x < tl) {
-      uint32_t y = s.nxt[x];
-      if (y == 0xffff || y <= x) {
-        bad = true;
-        break;
-      }
-      bytes += s.disk[x];
-      nb++;
-      x = y;
-    }
-    TileRow r;
-    r.exit = bad ? 0xffffffffu : x;  // window-relative; >= tile length unless the stream ended
-    r.nblk = nb;
-    r.bytes = bytes;
-    wk.rows[tile * hc + c] = r;
-  }
-  (void)err;
+  // exit window-relative: >= tile length unless the stream ended
+  for (uint32_t c = threadIdx.x; c < hc; c += kEncThreads) wk.rows[tile * hc + c] = follow_nxt(s.nxt, s.disk, c, tl);
   // ---- group completion: the last tile CTA of a group of kEncGroup tiles composes the group's transfer function and raises the
   // group's ready flag; the stitch kernel runs concurrently on its own stream and consumes the groups as they appear
   __threadfence();  // this thread's nxt / disk / rows stores are visible device-wide before the counter moves
@@ -558,11 +564,19 @@ __device__ __forceinline__ void close_file(FileRec* files, WalkState& st, uint64
 }
 // on-disk bytes of a data block that holds the single entry y
 __device__ __forceinline__ uint64_t single_entry_block_bytes(const KeyCols& m, const EncodeWork& wk, uint64_t y) {
-  uint32_t sh = wk.eshared[y], ks = meta_ulen(m.meta[y]) + 8;
-  uint64_t s0 = (uint64_t)wk.esz[y] + 1u + varint_len32(ks) + sh - varint_len32(sh) - varint_len32(ks - sh);
-  return s0 + 4 + 4 + 5;
+  return (uint64_t)wk.esz[y] + restart_surcharge(wk.eshared[y], meta_ulen(m.meta[y]) + 8) + 4 + 4 + 5;
 }
 // ---- grandparent boundaries on entry ranks: the state machine itself is gp_rules.h (host + device)
+// index of the first of the ncuts recorded cuts (sorted by entry) behind `entry`
+__device__ __forceinline__ uint32_t first_cut_after(const EncodeParams& ep, uint32_t ncuts, uint64_t entry) {
+  uint32_t lo = 0, hi = ncuts;
+  while (lo < hi) {
+    const uint32_t mid = (lo + hi) >> 1;
+    if (ep.gp_cuts[mid].entry <= entry) lo = mid + 1;
+    else hi = mid;
+  }
+  return lo;
+}
 // on-disk bytes (payload + trailer) of a block holding the entries [a, e): what BlockBuilder would have written had the block
 // been flushed there (every restart entry is stored with shared == 0)
 __device__ uint64_t truncated_block_bytes(const KeyCols& m, const EncodeWork& wk, uint32_t R, uint64_t a, uint64_t e) {
@@ -584,10 +598,7 @@ __device__ uint64_t truncated_block_bytes(const KeyCols& m, const EncodeWork& wk
       const uint64_t j = j0 + q;
       if (j < e) {
         sum += s1[q];
-        if ((j - a) % R == 0) {
-          const uint32_t ks = meta_ulen(mt[q]) + 8;
-          sum += 1u + varint_len32(ks) + sh[q] - varint_len32(sh[q]) - varint_len32(ks - sh[q]);
-        }
+        if ((j - a) % R == 0) sum += restart_surcharge(sh[q], meta_ulen(mt[q]) + 8);
       }
     }
   }
@@ -611,14 +622,7 @@ __device__ __forceinline__ bool chase_tile(const uint16_t* nxt, const uint32_t* 
   uint32_t ncuts = 0, cut_i = 0;
   if (kGp == 2) {
     ncuts = *ep.gp_ncuts;
-    // first recorded cut behind the current position
-    uint32_t lo = 0, hi = ncuts;
-    while (lo < hi) {
-      const uint32_t mid = (lo + hi) >> 1;
-      if (ep.gp_cuts[mid].entry <= st.a) lo = mid + 1;
-      else hi = mid;
-    }
-    cut_i = lo;
+    cut_i = first_cut_after(ep, ncuts, st.a);
   }
   const uint64_t tend = tstart + tl;
   const bool cut_files = ep.output_level != 0;
@@ -636,18 +640,12 @@ __device__ __forceinline__ bool chase_tile(const uint16_t* nxt, const uint32_t* 
       // entries a < e <= y are added while the block [a, y) is open: the flushed size they see is st.foff
       uint64_t cut_at = ~0ull, cut_bytes = 0;
       if (kGp == 1) {
-        uint64_t ev;
-        while ((ev = gp_next_event(g, ep.gp)) <= y && ev < n) {
-          const uint64_t prev_overlapped = g.overlapped;
-          const uint32_t crossed = gp_advance(g, ep.gp, ev);
-          if (ev > st.f_first_entry && gp_should_stop(g, ep.gp, crossed, prev_overlapped, st.foff)) {
-            cut_at = ev;
-            cut_bytes = ev == y ? (uint64_t)disk[x] : truncated_block_bytes(m, wk, ep.restart_interval, st.a, ev);
-            const uint32_t ci = *ep.gp_ncuts;
-            ep.gp_cuts[ci] = GpCut{cut_at, cut_bytes};
-            *ep.gp_ncuts = ci + 1;
-            break;
-          }
+        cut_at = gp_block_cut(g, ep.gp, y, n, st.foff);
+        if (cut_at != ~0ull) {
+          cut_bytes = cut_at == y ? (uint64_t)disk[x] : truncated_block_bytes(m, wk, ep.restart_interval, st.a, cut_at);
+          const uint32_t ci = *ep.gp_ncuts;
+          ep.gp_cuts[ci] = GpCut{cut_at, cut_bytes};
+          *ep.gp_ncuts = ci + 1;
         }
       } else if (cut_i < ncuts && ep.gp_cuts[cut_i].entry <= y) {
         cut_at = ep.gp_cuts[cut_i].entry;
@@ -664,7 +662,6 @@ __device__ __forceinline__ bool chase_tile(const uint16_t* nxt, const uint32_t* 
         st.f_first_entry = cut_at;
         st.f_first_blk = st.blk;
         st.a = cut_at;
-        if (kGp == 1) gp_file_started(g, ep.gp, cut_at);
         continue;
       }
     }
@@ -689,10 +686,7 @@ __device__ __forceinline__ bool chase_tile(const uint16_t* nxt, const uint32_t* 
       st.f_first_entry = y + 1;
       st.f_first_blk = st.blk;
       st.a = y + 1;
-      if (kGp == 1 && y + 1 < n) {  // ShouldStopBefore(y + 1) updated the boundary state before the size rule fired
-        gp_advance(g, ep.gp, y + 1);
-        gp_file_started(g, ep.gp, y + 1);
-      }
+      if (kGp == 1) gp_size_cut(g, ep.gp, y + 1, n);
     } else {
       st.a = y;
     }
@@ -774,9 +768,8 @@ encode_stitch_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t n, uint
       WalkState st = s.st;
       const GpState gps = s.gp;  // only read here: boundaries are crossed (and the state changes) inside chase_tile
       const uint64_t next_ev = ep.gp.n ? gp_next_event(gps, ep.gp) : ~0ull;
-      uint64_t cg = s.g, ct = s.t;
-      const uint64_t ctend_in = s.tend, cga = s.ga, cta = s.ta;
-      uint64_t ctend = ctend_in;
+      uint64_t cg = s.g, ct = s.t, ctend = s.tend;
+      const uint64_t cga = s.ga, cta = s.ta;
       const uint32_t cgn = s.gn, ctn = s.tn;
       uint32_t req = 0, fin = 0;
       uint64_t req_idx = 0;
@@ -792,25 +785,16 @@ encode_stitch_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t n, uint
             req_idx = t;
             break;
           }
-          TileState ts{st.a, st.blk, st.foff, st.f, 0};
-          wk.tstate[t] = ts;
+          wk.tstate[t] = TileState{st.a, st.blk, st.foff, st.f, 0};
           ct++;
           if (st.a >= tend) continue;  // no block starts in this tile
-          const uint64_t cc = st.a - tstart;
           TileRow r;
-          r.exit = 0xffffffffu;
-          if (cc < hc) r = tcache[(t - cta) * hc + cc];
-          const bool table_ok = cc < hc && r.exit != 0xffffffffu;
-          const bool cut = !table_ok || (ep.output_level != 0 && st.foff + r.bytes >= ep.max_output_file_size) || tstart + r.exit >= n ||
-                           next_ev <= tstart + r.exit;  // a grandparent boundary is crossed inside: the rules need the block-level state
-          if (cut) {  // a file ends in this tile (or the entry point is not tabulated): chase it block by block
-            req = 1;
+          if (must_descend(tabulated_row(tcache + (t - cta) * hc, st.a - tstart, hc, r), r, tstart, n, st.foff, ep, next_ev)) {
+            req = 1;  // chase the tile block by block
             req_idx = t;
             break;
           }
-          st.a = tstart + r.exit;
-          st.blk += r.nblk;
-          st.foff += r.bytes;
+          follow_row(r, tstart, st.a, st.blk, st.foff);
           continue;
         }
         // group level
@@ -826,27 +810,18 @@ encode_stitch_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t n, uint
           req_idx = gg;
           break;
         }
-        TileState gs{st.a, st.blk, st.foff, st.f, 0};
-        wk.gstate[gg] = gs;
+        wk.gstate[gg] = TileState{st.a, st.blk, st.foff, st.f, 0};
         wk.gflag[gg] = 0;
         cg++;
         if (st.a >= gend) continue;  // no block starts in this group
-        const uint64_t cc = st.a - gstart;
         TileRow r;
-        r.exit = 0xffffffffu;
-        if (cc < hc) r = gcache[(gg - cga) * hc + cc];
-        const bool table_ok = cc < hc && r.exit != 0xffffffffu;
-        const bool cut = !table_ok || (ep.output_level != 0 && st.foff + r.bytes >= ep.max_output_file_size) || gstart + r.exit >= n ||
-                         next_ev <= gstart + r.exit;
-        if (cut) {  // descend: tile by tile
-          wk.gflag[gg] = 1;
+        if (must_descend(tabulated_row(gcache + (gg - cga) * hc, st.a - gstart, hc, r), r, gstart, n, st.foff, ep, next_ev)) {
+          wk.gflag[gg] = 1;  // walk the group tile by tile
           ct = t0;
           ctend = t1;
           continue;
         }
-        st.a = gstart + r.exit;
-        st.blk += r.nblk;
-        st.foff += r.bytes;
+        follow_row(r, gstart, st.a, st.blk, st.foff);
       }
       s.st = st;
       s.g = cg;
@@ -1006,19 +981,12 @@ __global__ void encode_tilestate_kernel(EncodeWork wk, uint64_t n, uint64_t ntil
     TileState ts{a < n ? a : n, blk, foff, gs.file_idx, 0};
     wk.tstate[t] = ts;
     if (a >= n || a >= tend) continue;
-    const uint64_t cc = a - tstart;
-    if (cc >= hc) {
+    TileRow r;
+    if (!tabulated_row(wk.rows + t * hc, a - tstart, hc, r)) {
       atomicOr(err, kErrBlockTooLong);
       return;
     }
-    const TileRow r = wk.rows[t * hc + cc];
-    if (r.exit == 0xffffffffu) {
-      atomicOr(err, kErrBlockTooLong);
-      return;
-    }
-    a = tstart + r.exit;
-    blk += r.nblk;
-    foff += r.bytes;
+    follow_row(r, tstart, a, blk, foff);
   }
 }
 
@@ -1045,34 +1013,17 @@ encode_blocklist_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t n, u
   }
   __syncthreads();
   if (threadIdx.x == 0) {
-    // follow the chain; decide whether a file ends inside this tile
-    uint32_t x = (uint32_t)(ts.entry - tstart);
-    uint64_t bytes = 0;
-    bool bad = false, ends = false;
-    while (x < tl) {
-      uint32_t y = s.nxt[x];
-      if (y == 0xffff || y <= x) {
-        bad = true;
-        break;
-      }
-      s.is_start[x] = 1;
-      bytes += s.disk[x];
-      if (tstart + y >= n) ends = true;
-      x = y;
-    }
+    // follow the chain, marking the block starts; a file ends inside this tile when the stitch walk would have descended into it,
+    // with the recorded grandparent cuts in place of the rules' events
+    const TileRow r = follow_nxt(s.nxt, s.disk, (uint32_t)(ts.entry - tstart), tl, s.is_start);
+    const bool bad = r.exit == 0xffffffffu;
     if (bad) atomicOr(err, kErrBlockTooLong);
-    bool gp_cut = false;  // a recorded grandparent cut inside this tile's chain (ts.entry, x]
+    uint64_t next_cut = ~0ull;
     if (ep.gp.n && !bad) {
-      const uint32_t nc = *ep.gp_ncuts;
-      uint32_t lo = 0, hi = nc;
-      while (lo < hi) {
-        const uint32_t mid = (lo + hi) >> 1;
-        if (ep.gp_cuts[mid].entry <= ts.entry) lo = mid + 1;
-        else hi = mid;
-      }
-      gp_cut = lo < nc && ep.gp_cuts[lo].entry <= tstart + x;
+      const uint32_t nc = *ep.gp_ncuts, ci = first_cut_after(ep, nc, ts.entry);
+      if (ci < nc) next_cut = ep.gp_cuts[ci].entry;
     }
-    s.serial = bad ? 2 : ((ends || gp_cut || (ep.output_level != 0 && ts.file_off + bytes >= ep.max_output_file_size)) ? 1 : 0);
+    s.serial = bad ? 2 : must_descend(true, r, tstart, n, ts.file_off, ep, next_cut) ? 1 : 0;
     if (s.serial == 1) {  // an output file ends inside this tile: replay the exact serial rule
       WalkState st;
       st.a = ts.entry;
@@ -2266,8 +2217,7 @@ void launch_encode_sizes(KeyCols m, const unsigned long long* n_dev, EncodeWork 
   const uint64_t tiles = (n_cap + kEncTile - 1) / kEncTile;
   encode_sizes_kernel<<<(unsigned)(tiles < (unsigned)sms * 8 ? tiles : (unsigned)sms * 8), 256, 0, st>>>(m, n_dev, w.esz, w.eshared, w.tstat, tprefix_out, w.min_s1);
 }
-void launch_encode_tables(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t ntiles, uint32_t hc, uint32_t max_s1, uint32_t* err,
-                          cudaStream_t st) {
+void launch_encode_tables(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t ntiles, uint32_t hc, uint32_t max_s1, cudaStream_t st) {
   if (ntiles == 0) return;
   static PerDeviceFlag attr;
   const uint64_t dev_bit = attr.bit_of_current_device();
@@ -2278,9 +2228,9 @@ void launch_encode_tables(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nti
   }
   // all prefix sums of a window stay below 2^32 when (largest entry) x (window length) does
   if (((uint64_t)max_s1 + 64) * (uint64_t)(kW + 1) < (1ull << 32))
-    encode_tables_kernel<uint32_t><<<(unsigned)ntiles, kEncThreads, sizeof(TablesSmem<uint32_t>), st>>>(m, ep, w, m.n, hc, w.nxt, w.disk, err);
+    encode_tables_kernel<uint32_t><<<(unsigned)ntiles, kEncThreads, sizeof(TablesSmem<uint32_t>), st>>>(m, ep, w, m.n, hc);
   else
-    encode_tables_kernel<uint64_t><<<(unsigned)ntiles, kEncThreads, sizeof(TablesSmem<uint64_t>), st>>>(m, ep, w, m.n, hc, w.nxt, w.disk, err);
+    encode_tables_kernel<uint64_t><<<(unsigned)ntiles, kEncThreads, sizeof(TablesSmem<uint64_t>), st>>>(m, ep, w, m.n, hc);
 }
 void launch_encode_stitch(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t ntiles, uint32_t hc, uint32_t* err, uint32_t attempt,
                           uint32_t* sflag, cudaStream_t st, uint64_t* launches) {

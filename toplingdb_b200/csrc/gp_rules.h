@@ -88,4 +88,30 @@ B200C_HD void gp_file_started(GpState& g, const GpCtx& c, uint64_t e) {
   g.overlapped = gp_overlap_at(g, c, e);
 }
 
+// The two steps of the output-file walk over a stream of n entries (encode.cu chase_tile; tests/native/gp_rules_sim.cc).
+// The entries a < e <= end are added while one block is open and `cur` bytes are flushed to the file: crosses the boundaries up to
+// `end` and returns the first entry in front of which the rules end the file (the boundary state is then the next file's), or ~0.
+// Every event seen here lies behind the open file's first entry: each file start was passed to gp_advance (the stream's first entry
+// before the walk, the cut returned here, the entry behind gp_size_cut's), and gp_next_event is always beyond the last entry
+// advanced to.  So the rules never stop in front of a file's first key, and no guard for that is needed.
+B200C_HD uint64_t gp_block_cut(GpState& g, const GpCtx& c, uint64_t end, uint64_t n, uint64_t cur) {
+  uint64_t ev;
+  while ((ev = gp_next_event(g, c)) <= end && ev < n) {
+    const uint64_t prev_overlapped = g.overlapped;
+    const uint32_t crossed = gp_advance(g, c, ev);
+    if (gp_should_stop(g, c, crossed, prev_overlapped, cur)) {
+      gp_file_started(g, c, ev);
+      return ev;
+    }
+  }
+  return ~0ull;
+}
+// the size rule closed the file behind entry e - 1 (:277): ShouldStopBefore(e) moved the boundary state before the rule fired, and
+// entry e starts the next file
+B200C_HD void gp_size_cut(GpState& g, const GpCtx& c, uint64_t e, uint64_t n) {
+  if (e >= n) return;
+  gp_advance(g, c, e);
+  gp_file_started(g, c, e);
+}
+
 }  // namespace b200c

@@ -197,8 +197,8 @@ struct TileState {           // resolved state when the chain enters a tile
   uint32_t pad;
 };
 constexpr int kEncTile = 4096;       // entries per block-cut tile
-constexpr int kEncHalo = 2048;
-constexpr int kEncGroupTiles = 16;   // tiles per stitch group (encode.cu kEncGroup)       // look-ahead window = the longest block (in entries) the encoder accepts
+constexpr int kEncHalo = 2048;       // look-ahead window = the longest block (in entries) the encoder accepts
+constexpr int kEncGroupTiles = 16;   // tiles per stitch group (encode.cu kEncGroup)
 constexpr uint32_t kMaxOutFiles = 4096;
 
 struct EncodeWork {                  // device scratch owned by the job
@@ -230,8 +230,7 @@ struct EncodeWork {                  // device scratch owned by the job
 };
 // TableBuilder-only path (no merge in front): sizes + statistics per kEncTile entries + their prefix array (tprefix_out)
 void launch_encode_sizes(KeyCols m, const unsigned long long* n_dev, EncodeWork w, unsigned long long* tprefix_out, uint64_t n_cap, int sms, cudaStream_t st);
-void launch_encode_tables(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t ntiles, uint32_t hc, uint32_t max_s1, uint32_t* err,
-                          cudaStream_t st);
+void launch_encode_tables(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t ntiles, uint32_t hc, uint32_t max_s1, cudaStream_t st);
 // stitch: launched on its own stream BEFORE / alongside launch_encode_tables (it consumes groups as their gready flag appears);
 // tilestate: after both have finished
 void launch_encode_stitch(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t ntiles, uint32_t hc, uint32_t* err, uint32_t attempt,
