@@ -95,3 +95,45 @@ def parse_key_recs(b):
         uk = struct.pack(">QQ", hi, lo)[:ulen]
         out.append((uk, tr, vlen))
     return out
+
+
+def describe_first_difference(got, want):
+    """Names the region of the first byte where `got` differs from the oracle's file `want`, from the layout of `want`: data block i,
+    filter slice s and line, filter metadata / trailer, index entry b (with the oracle's separator key and handle), index restart
+    array / trailer, properties, metaindex or footer."""
+    import sstfmt
+    j = next((i for i in range(min(len(got), len(want))) if got[i] != want[i]), min(len(got), len(want)))
+    head = f"byte {j} of {len(want)} (device file: {len(got)} bytes)"
+    ft = sstfmt.parse_footer(want)
+    mo, ms = ft["metaindex"]
+    io, isz = ft["index"]
+    regions = [(len(want) - 53, len(want), "footer"), (mo, mo + ms + 5, "metaindex block")]
+    mblock, _, _ = sstfmt.read_block(want, ft["metaindex"])
+    for k, v, _ in sstfmt.block_entries(mblock):
+        o, q = sstfmt.varint(v, 0)
+        s, q = sstfmt.varint(v, q)
+        name = k.decode()
+        if name.startswith("fullfilter."):
+            from index_filter_cases import SLICE as slice_bytes  # kBloomSliceBytes, read out of csrc/encode.cu
+            if o <= j < o + s - 5:
+                return f"{head}: filter bits, slice {(j - o) // slice_bytes}, line {(j - o) // 64} (byte {(j - o) % 64} of the line)"
+            regions += [(o + s - 5, o + s, "filter metadata"), (o + s, o + s + 5, "filter block trailer")]
+        else:
+            regions.append((o, o + s + 5, f"{name} block"))
+    iblock, _, _ = sstfmt.read_block(want, ft["index"])
+    nr = struct.unpack_from("<I", iblock, len(iblock) - 4)[0]
+    restarts = [struct.unpack_from("<I", iblock, len(iblock) - 4 - 4 * nr + 4 * b)[0] for b in range(nr)]
+    ends = restarts[1:] + [len(iblock) - 4 - 4 * nr]
+    handles = [h for _, h in sstfmt.parse_sst(want)["index"]]
+    for b, (a, e) in enumerate(zip(restarts, ends)):  # index restart interval 1: every entry is a restart point
+        if io + a <= j < io + e:
+            (key, _, _), = sstfmt.block_entries(iblock[a:e] + struct.pack("<II", 0, 1), value_delta=ft["format_version"] >= 4)
+            return f"{head}: index entry {b} of {nr}, oracle separator {key.hex() or '(empty)'} handle {handles[b]}"
+    regions += [(io + ends[-1] if ends else io, io + isz, "index restart array"), (io + isz, io + isz + 5, "index block trailer")]
+    for a, e, what in regions:
+        if a <= j < e:
+            return f"{head}: {what}"
+    for i, (o, s) in enumerate(handles):
+        if o <= j < o + s + 5:
+            return f"{head}: data block {i} (offset {o}, {s} bytes + trailer)"
+    return f"{head}: outside every block of the oracle's file"

@@ -314,7 +314,7 @@ int map_dev_err(uint32_t e) {
   if (e & kErrParanoid) m += " Paranoid checksums do not match (an output file does not read back as written)";
   if (e & kErrSingleDelContract) m += " SingleDelete and Delete of the same key in one snapshot stripe (enforce_single_del_contracts)";
   const uint32_t unsup = kErrKeyTooLong | kErrValueTooLong | kErrBadType | kErrCompressed | kErrBlockTooLong | kErrIrregularRestarts |
-                         kErrGroupTooLong | kErrSdWriteConflict;
+                         kErrGroupTooLong | kErrSdWriteConflict | kErrTooManyFiles;
   if (e & unsup) {
     if (!(e & ~(unsup))) code = B200C_ERR_NOT_SUPPORTED;
     if (e & kErrKeyTooLong) m += " user-key-longer-than-16-bytes";
@@ -325,6 +325,7 @@ int map_dev_err(uint32_t e) {
     if (e & kErrCompressed) m += " compressed-block";
     if (e & kErrBlockTooLong) m += " output-block-with-too-many-entries";
     if (e & kErrIrregularRestarts) m += " restart-intervals-of-unequal-length";
+    if (e & kErrTooManyFiles) m += " more-than-" + std::to_string(kMaxOutFiles) + "-output-files";
   }
   if (e & kErrInternal) {
     m += " internal";

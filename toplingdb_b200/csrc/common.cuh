@@ -28,6 +28,7 @@ enum DevErr : uint32_t {
   kErrSingleDelContract = 1u << 12,  // a SingleDelete met a Delete of the same key in one snapshot stripe (enforce_single_del_contracts)
   kErrGroupTooLong = 1u << 13,   // a user key with a SingleDelete has more versions than the device walks serially
   kErrSdWriteConflict = 1u << 14,  // SingleDelete with an earliest_write_conflict_snapshot (transaction DB): not on the device
+  kErrTooManyFiles = 1u << 15,   // the job cuts more output files than the encoder's file records hold (kMaxOutFiles)
   // not an error: some input entry is a kTypeSingleDeletion (the merge then keeps every user key's versions inside one tile)
   kFlagHasSingleDelete = 1u << 31,
 };

@@ -545,8 +545,8 @@ struct WalkState {
 };
 __device__ __forceinline__ void close_file(FileRec* files, WalkState& st, uint64_t end_entry, uint32_t* err) {
   if (files == nullptr) return;  // block-list pass: the stitch kernel already wrote the file records
-  if (st.f >= kMaxOutFiles) {
-    atomicOr(err, kErrInternal);
+  if (st.f >= kMaxOutFiles) {  // a documented limit of the device rule set, not a fault: nothing is written past the records
+    atomicOr(err, kErrTooManyFiles);
     return;
   }
   FileRec& fr = files[st.f];
