@@ -142,6 +142,16 @@ typedef struct b200c_params {
    * what happens to a SingleDelete (compaction_iterator.cc:801-838); with one set (transaction DBs) an input that holds a
    * SingleDelete is answered with B200C_ERR_NOT_SUPPORTED. */
   uint64_t earliest_write_conflict_snapshot;
+  /* ColumnFamilyOptions::sst_partitioner_factory = NewSstPartitionerFixedPrefixFactory(len): the prefix length, 0 = no partitioner.
+   * Appended to the struct (the ABI version did not change): a caller that zero-initialises it, or leaves it as b200c_params_init
+   * sets it, keeps the old behaviour.  An output file never holds two user keys whose first `len` bytes differ: CompactionOutputs::
+   * ShouldStopBefore (db/compaction/compaction_outputs.cc:264-269) ends the file in front of every output entry whose user key,
+   * truncated to len bytes (a shorter key stays whole), differs from the previous output entry's (SstPartitionerFixedPrefix::
+   * ShouldPartition, db/compaction/sst_partitioner.cc) -- before the size and grandparent rules, never at a file's first entry.
+   * Ignored when output_level == 0 (no partitioner for L0 outputs, compaction_outputs.cc:793-795).  A job whose partition cuts alone
+   * would give more output files than the device's file records hold (4096) is answered with B200C_ERR_NOT_SUPPORTED before any
+   * file is written. */
+  uint32_t sst_partitioner_prefix_len;
 } b200c_params;
 
 /* FileMinMeta (compaction_executor.h:120-131) + the TableProperties RunRemote re-reads (compaction_job.cc:1043-1061) */

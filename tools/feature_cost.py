@@ -1,6 +1,9 @@
 """Measures what the optional parts of the compaction path cost on the bench workload (BASELINE.json configs[1], cfg2: 8 x 256 MiB runs,
-16 B keys / 32 B values): the same job with a Bloom filter policy, with paranoid_file_checks, with grandparent files, and clipped to a
-quarter of the key space, each timed on the device with the per-kernel events of `profile=1`.  Prints one JSON object:
+16 B keys / 32 B values): the same job with a Bloom filter policy, with paranoid_file_checks, with grandparent files, clipped to a
+quarter of the key space, and with a fixed-prefix SST partitioner, each timed on the device with the per-kernel events of `profile=1`.
+cfg2's keys share their first byte, split into ~580 groups on their first 3 bytes and are unique in their first 8: the partitioner arms
+are a job the walk descends into nowhere (len 1), one with ~580 partition cuts (len 3), and one the device refuses (len 8: an event at
+every entry), timed from the run call to the refusal.  Prints one JSON object:
 `python tools/feature_cost.py > feature_cost.json` on the GPU to be measured."""
 import json
 import os
@@ -38,6 +41,8 @@ def main():
         "grandparents_64": dict(grandparents=gps, max_output_file_size=128 << 20, target_output_file_size=64 << 20,
                                 level_compaction_dynamic_file_size=1),
         "range_second_quarter": dict(range_start=key(n_total // 4), range_end=key(n_total // 2)),
+        "partitioner_len1": dict(sst_partitioner_prefix_len=1),
+        "partitioner_len3": dict(sst_partitioner_prefix_len=3),
     }
     out = {"workload": "cfg2", "scale": scale, "input_kv_bytes": kv_bytes, "variants": {}}
     for name, extra in variants.items():
@@ -59,6 +64,21 @@ def main():
             "kernels_us": {kn: round(statistics.mean(v), 1) for kn, v in sorted(kt.items(), key=lambda x: -statistics.mean(x[1]))}}
         job.close()
         torch.cuda.synchronize()
+    import time
+    job = T.CompactionJob(**dict(common, sst_partitioner_prefix_len=8))
+    for i, img in enumerate(images):
+        job.add_input(img, level=0, file_number=100 + i)
+    refusal = []
+    for _ in range(3):
+        t0 = time.perf_counter()
+        try:
+            job.run()
+            code = 0
+        except T.B200cError as e:
+            code = e.code
+        refusal.append((time.perf_counter() - t0) * 1e6)
+    out["variants"]["partitioner_len8_refused"] = {"status": code, "wall_us_to_refusal": round(statistics.mean(refusal), 1)}
+    job.close()
     print(json.dumps(out))
 
 

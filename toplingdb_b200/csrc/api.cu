@@ -266,6 +266,7 @@ struct b200c_job {
   std::vector<uint64_t> gp_size;
   std::vector<uint8_t> gp_same;
   DevBuf gp_keys_d, gp_ranks_d, gp_size_d, gp_same_d, gp_cuts_d;
+  DevBuf pev_d;  // fixed-prefix partitioner: event entries, look-back ticket and state
   BoundKey range_lo{}, range_hi{};  // sub-compaction key range in column form (has_range_start / has_range_end in p)
   DevBuf clip_d;                    // clipped run bounds: begin[k] | end[k]
   DevBuf cslot, cslot_off, arena;   // compressed inputs: arena slot size / offset per data block, the inflated blocks
@@ -673,14 +674,15 @@ int encode_stage(b200c_job* j, KeyCols mcols, uint64_t n_out, uint32_t min_s1, u
     ep.format_version = P.format_version;
     ep.output_level = (uint32_t)P.output_level;
     ep.max_output_file_size = P.max_output_file_size;
-    if (!j->gp_small.empty() && P.output_level > 0) {
+    // L0 outputs are never cut by grandparents or a partitioner (compaction_outputs.cc:247-253, :793-795)
+    const uint32_t G = P.output_level > 0 ? (uint32_t)j->gp_small.size() : 0;
+    const uint32_t plen = P.output_level > 0 ? P.sst_partitioner_prefix_len : 0;
+    if (G) {
       // grandparent boundaries -> ranks in the merged stream; the cut rules themselves run inside the stitch kernel
-      const uint32_t G = (uint32_t)j->gp_small.size();
       CU(j->gp_keys_d.reserve(sizeof(GpKey) * 2 * G));
       CU(j->gp_ranks_d.reserve(8 * 3 * (size_t)G));
       CU(j->gp_size_d.reserve(8 * (size_t)G));
       CU(j->gp_same_d.reserve(G + 16));
-      CU(j->gp_cuts_d.reserve(sizeof(GpCut) * (2 * (size_t)G + 2)));
       GpKey* keys = j->gp_keys_d.as<GpKey>();
       if (int rc = upload_small(j, keys, j->gp_small.data(), sizeof(GpKey) * G)) return rc;
       if (int rc = upload_small(j, keys + G, j->gp_large.data(), sizeof(GpKey) * G)) return rc;
@@ -698,6 +700,25 @@ int encode_stage(b200c_job* j, KeyCols mcols, uint64_t n_out, uint32_t min_s1, u
       ep.gp.next_same = j->gp_same_d.as<uint8_t>();
       ep.gp.target_output_file_size = P.target_output_file_size ? P.target_output_file_size : P.max_output_file_size;
       ep.gp.max_compaction_bytes = P.max_compaction_bytes ? P.max_compaction_bytes : ep.gp.target_output_file_size * 25;
+    }
+    if (plen) {
+      // the partition events as a sorted entry list: k events make k + 1 files, so kMaxOutFiles - 1 of them fill the file records
+      const uint32_t cap = kMaxOutFiles - 1;
+      const uint64_t ptiles = partition_event_tiles(n_out);
+      CU(j->pev_d.reserve(8 * ((size_t)cap + 1 + ptiles)));
+      uint64_t* pev = j->pev_d.as<uint64_t>();  // events [cap] | look-back ticket | look-back state [ptiles]
+      CU(cudaMemsetAsync(pev, 0xff, 8 * (size_t)cap, st));
+      CU(cudaMemsetAsync(pev + cap, 0, 8 * (1 + ptiles), st));
+      j->kt_begin("encode.partition_events");
+      launch_partition_events(mcols, plen, cap, reinterpret_cast<uint32_t*>(pev + cap), reinterpret_cast<unsigned long long*>(pev + cap + 1),
+                              pev, err, st);
+      j->kt_end();
+      j->launches += 1;
+      ep.gp.pev = pev;
+      ep.gp.np = cap;
+    }
+    if (G || plen) {  // every cut the stitch walk makes by these rules, for the block-list kernel: at most two per grandparent + the events
+      CU(j->gp_cuts_d.reserve(sizeof(GpCut) * (2 * (size_t)G + 2 + ep.gp.np)));
       ep.gp_cuts = j->gp_cuts_d.as<GpCut>();
       ep.gp_ncuts = reinterpret_cast<uint32_t*>(small + kSlotGpCuts);
     }

@@ -433,7 +433,7 @@ __device__ __forceinline__ TileRow follow_nxt(const uint16_t* nxt, const uint32_
 }
 // The one descend rule of the stitch walk and the block list: a span cannot be crossed by its row r (from the chain position
 // whose file holds `foff` bytes) when the row is not tabulated, the size rule fires inside, the stream ends inside, or a grandparent
-// boundary (next_ev: the next event of the rules, or in the block list the next recorded cut) lies inside.
+// boundary or partition event (next_ev: the next event of the rules, or in the block list the next recorded cut) lies inside.
 __device__ __forceinline__ bool must_descend(bool tabulated, const TileRow& r, uint64_t start, uint64_t n, uint64_t foff,
                                              const EncodeParams& ep, uint64_t next_ev) {
   return !tabulated || (ep.output_level != 0 && foff + r.bytes >= ep.max_output_file_size) || start + r.exit >= n ||
@@ -609,7 +609,7 @@ __device__ uint64_t truncated_block_bytes(const KeyCols& m, const EncodeWork& wk
 // Follow the real chain through one tile whose nxt/disk sit in shared memory, applying the output-file cut rules
 // (compaction_outputs.cc:277: cut in front of the first entry added after the flushed size reached the maximum; :294-351 the
 // grandparent rules).  emit != nullptr: write BlockRecs.  files != nullptr: write FileRecs.
-// kGp: 0 = no grandparents; 1 = evaluate the grandparent rules (stitch; records the cuts); 2 = replay recorded cuts (block list).
+// kGp: 0 = no grandparents or partitioner; 1 = evaluate their rules (stitch; records the cuts); 2 = replay recorded cuts (block list).
 // The walk state is copied into registers for the loop (taking its address would put it in local memory and turn every
 // step of this single-thread pointer chase into a chain of dependent local loads and stores).
 template <int kGp>
@@ -751,7 +751,7 @@ encode_stitch_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t n, uint
   if (threadIdx.x == 0) {
     s.st = WalkState{0, 0, 0, 0, 0, 0};
     s.gp = gp_initial_state();
-    if (ep.gp.n) {
+    if (gp_rules_on(ep.gp)) {
       *ep.gp_ncuts = 0;
       if (n) gp_advance(s.gp, ep.gp, 0);  // ShouldStopBefore of the first key: no builder yet, but the boundary state moves
     }
@@ -767,7 +767,7 @@ encode_stitch_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t n, uint
       // everything the serial walk touches per step lives in registers; shared memory is read / written once per section
       WalkState st = s.st;
       const GpState gps = s.gp;  // only read here: boundaries are crossed (and the state changes) inside chase_tile
-      const uint64_t next_ev = ep.gp.n ? gp_next_event(gps, ep.gp) : ~0ull;
+      const uint64_t next_ev = gp_rules_on(ep.gp) ? gp_next_event(gps, ep.gp) : ~0ull;
       uint64_t cg = s.g, ct = s.t, ctend = s.tend;
       const uint64_t cga = s.ga, cta = s.ta;
       const uint32_t cgn = s.gn, ctn = s.tn;
@@ -890,7 +890,7 @@ encode_stitch_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t n, uint
       coop_copy_cg<uint4, 4>(reinterpret_cast<uint4*>(s.nxt + c0), reinterpret_cast<const uint4*>(wk.nxt + tstart + c0), (c1 - c0) / 8);
       coop_copy_cg<uint4, 8>(reinterpret_cast<uint4*>(s.disk + c0), reinterpret_cast<const uint4*>(wk.disk + tstart + c0), (c1 - c0) / 4);
       __syncthreads();
-      if (ep.gp.n == 0) {
+      if (!gp_rules_on(ep.gp)) {
         for (uint32_t i = c0 + threadIdx.x; i < tl; i += blockDim.x) s.nd[i] = ((uint64_t)s.nxt[i] << 32) | s.disk[i];
         __syncthreads();
       }
@@ -898,10 +898,10 @@ encode_stitch_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t n, uint
         WalkState st = s.st;
         GpState g = s.gp;
         bool chased = true;
-        if (ep.gp.n) {
+        if (gp_rules_on(ep.gp)) {
           chased = chase_tile<1>(s.nxt, s.disk, tstart, tl, n, ep, m, wk, st, wk.files, nullptr, 0, err, &g);
         } else {
-          // Without grandparents the only events on the chain are the size rule and the end of the stream.  The walk is one thread
+          // Without grandparents or a partitioner the only events on the chain are the size rule and the end of the stream.  The walk is one thread
           // chasing dependent loads, so the common link is kept to a single 8-byte shared-memory load and a dozen 32-bit instructions
           // (the general loop costs ~320 cycles per link, measured with clock64: 58 links per file cut); the block in which an event
           // happens goes through the exact rule (chase_tile over that one block).
@@ -1019,7 +1019,7 @@ encode_blocklist_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t n, u
     const bool bad = r.exit == 0xffffffffu;
     if (bad) atomicOr(err, kErrBlockTooLong);
     uint64_t next_cut = ~0ull;
-    if (ep.gp.n && !bad) {
+    if (gp_rules_on(ep.gp) && !bad) {
       const uint32_t nc = *ep.gp_ncuts, ci = first_cut_after(ep, nc, ts.entry);
       if (ci < nc) next_cut = ep.gp_cuts[ci].entry;
     }
@@ -1032,7 +1032,7 @@ encode_blocklist_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t n, u
       st.f = ts.file_idx;
       st.f_first_entry = 0;
       st.f_first_blk = 0;
-      const bool chased = ep.gp.n ? chase_tile<2>(s.nxt, s.disk, tstart, tl, n, ep, m, wk, st, nullptr, wk.blocks, nblk_cap, err)
+      const bool chased = gp_rules_on(ep.gp) ? chase_tile<2>(s.nxt, s.disk, tstart, tl, n, ep, m, wk, st, nullptr, wk.blocks, nblk_cap, err)
                                   : chase_tile<0>(s.nxt, s.disk, tstart, tl, n, ep, m, wk, st, nullptr, wk.blocks, nblk_cap, err);
       if (!chased) atomicOr(err, kErrBlockTooLong);
     }
@@ -2174,6 +2174,76 @@ __global__ void gp_rank_kernel(KeyCols m, const GpKey* __restrict__ smallest, co
 void launch_gp_ranks(KeyCols m, const GpKey* smallest, const GpKey* largest, uint32_t n, uint64_t* lo, uint64_t* eq, uint64_t* hi,
                      cudaStream_t st) {
   if (n) gp_rank_kernel<<<(n + 63) / 64, 64, 0, st>>>(m, smallest, largest, n, lo, eq, hi);
+}
+
+// ---- fixed-prefix SST partitioner (SstPartitionerFixedPrefix::ShouldPartition, db/compaction/sst_partitioner.cc): entry e >= 1
+// of the merged stream is an event when its user key and entry e - 1's, each truncated to len bytes (a shorter key stays whole),
+// differ.  The merged stream is exactly what the reference adds to its outputs (last_key_for_partitioner_, compaction_outputs.cc:
+// 394-398), so dropped versions never count.  Keys are at most 16 bytes: the compare is one on the (hi, lo) words under a byte mask.
+__device__ __forceinline__ bool partition_prefix_differs(ulonglong2 a, uint32_t alen, ulonglong2 b, uint32_t blen, uint32_t len) {
+  const uint32_t la = alen < len ? alen : len, lb = blen < len ? blen : len;
+  if (la != lb) return true;
+  const uint64_t mhi = la >= 8 ? ~0ull : (la ? ~0ull << (64 - 8 * la) : 0ull);
+  const uint64_t mlo = la >= 16 ? ~0ull : (la > 8 ? ~0ull << (64 - 8 * (la - 8)) : 0ull);
+  return (((a.x ^ b.x) & mhi) | ((a.y ^ b.y) & mlo)) != 0;
+}
+constexpr int kPevThreads = 256, kPevItems = 8, kPevTile = kPevThreads * kPevItems;
+// One CTA per kPevTile entries, taken in ticket order: flag every entry, count per warp and round, find the CTA's first event rank by
+// the decoupled look-back over the CTAs in front, then write the events in entry order.  Ranks >= cap (more files than the encoder's
+// records hold) are not stored; they mark the job kErrTooManyFiles, which the host reads before any file is written.
+__global__ void __launch_bounds__(kPevThreads)
+partition_events_kernel(KeyCols m, uint32_t len, uint32_t cap, uint32_t* __restrict__ ticket, unsigned long long* __restrict__ state,
+                        uint64_t* __restrict__ ev, uint32_t* __restrict__ err) {
+  constexpr int kWarps = kPevThreads / 32;
+  __shared__ uint32_t s_tile, s_off[kPevItems][kWarps];
+  __shared__ uint64_t s_base;
+  if (threadIdx.x == 0) s_tile = atomicAdd(ticket, 1u);
+  __syncthreads();
+  const uint64_t t0 = (uint64_t)s_tile * kPevTile;
+  const unsigned lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  uint32_t flags = 0;
+#pragma unroll
+  for (int i = 0; i < kPevItems; i++) {  // round i: the CTA's threads on kPevThreads consecutive entries
+    const uint64_t e = t0 + (uint64_t)i * kPevThreads + threadIdx.x;
+    bool f = false;
+    if (e >= 1 && e < m.n) f = partition_prefix_differs(m.pfx[e - 1], meta_ulen(m.meta[e - 1]), m.pfx[e], meta_ulen(m.meta[e]), len);
+    const unsigned b = __ballot_sync(0xffffffffu, f);
+    if (lane == 0) s_off[i][w] = __popc(b);
+    flags |= (uint32_t)f << i;
+  }
+  __syncthreads();
+  if (w == 0) {
+    uint32_t total = 0;
+    if (lane == 0) {  // (round, warp) order is entry order: exclusive offsets of the 64 counts
+      for (int i = 0; i < kPevItems; i++)
+        for (int k = 0; k < kWarps; k++) {
+          const uint32_t c = s_off[i][k];
+          s_off[i][k] = total;
+          total += c;
+        }
+      lb_publish(state, s_tile, total);
+    }
+    total = __shfl_sync(0xffffffffu, total, 0);
+    const uint64_t base = lb_exclusive_prefix(state, s_tile, total, lane, 64);
+    if (lane == 0) s_base = base;
+  }
+  __syncthreads();
+  const uint64_t base = s_base;
+#pragma unroll
+  for (int i = 0; i < kPevItems; i++) {
+    const bool f = (flags >> i) & 1u;
+    const unsigned b = __ballot_sync(0xffffffffu, f);
+    if (!f) continue;
+    const uint64_t r = base + s_off[i][w] + __popc(b & ((1u << lane) - 1u));
+    if (r < cap) ev[r] = t0 + (uint64_t)i * kPevThreads + threadIdx.x;
+    else atomicOr(err, kErrTooManyFiles);
+  }
+}
+uint64_t partition_event_tiles(uint64_t n) { return (n + kPevTile - 1) / kPevTile; }
+void launch_partition_events(KeyCols m, uint32_t len, uint32_t cap, uint32_t* ticket, unsigned long long* state, uint64_t* ev, uint32_t* err,
+                             cudaStream_t st) {
+  const uint64_t tiles = partition_event_tiles(m.n);
+  if (tiles) partition_events_kernel<<<(unsigned)tiles, kPevThreads, 0, st>>>(m, len, cap, ticket, state, ev, err);
 }
 
 // file tails (properties | metaindex | footer, built on the host) from their staging buffer into the output images

@@ -5,6 +5,12 @@
 // `e < lo_i`, `e < eq_i` / `eq_i <= e < hi_i`, `e < lo_{i+1}` for the merged entry e (GpCtx, kernels.h), so the state machine only
 // has to run at the entries where a rank is reached.  Host + device: the encoder's stitch walk (encode.cu, chase_tile) runs it on
 // the GPU, tests/native/gp_rules_sim.cc runs the same code on the CPU against the oracle's file boundaries.
+//
+// A second source of events, checked before the size and grandparent rules (ShouldStopBefore :264-269): the fixed-prefix SST
+// partitioner (SstPartitionerFixedPrefix::ShouldPartition, db/compaction/sst_partitioner.cc) cuts in front of every output
+// entry whose user key, truncated to the prefix length, differs from the previous output entry's.  That is a function of the merged
+// stream alone, so the entries are listed once (partition_events_kernel, encode.cu) and the walk meets them like grandparent events.
+// tests/native/partition_rules_sim.cc runs them on the CPU.
 #pragma once
 #include <stdint.h>
 
@@ -25,18 +31,26 @@ struct GpCtx {
   const uint64_t* size;        // [n] file sizes
   const uint8_t* next_same;    // [n] smallest_{i+1} == largest_i (the key spans both files)
   uint64_t max_compaction_bytes, target_output_file_size;
+  const uint64_t* pev;         // [np] ascending entries in front of which the partitioner cuts; ~0 past the last one
+  uint32_t np;                 // slots of pev (0: no partitioner)
 };
 
 struct GpState {               // compaction_outputs.h:331-372 (being_grandparent_gap_, seen_key_, grandparent_index_, ...)
-  uint32_t being_gap, seen, index, pad;
+  uint32_t being_gap, seen, index, part;  // part: next partition event (pev index)
   uint64_t overlapped, switched;
 };
 B200C_HD GpState gp_initial_state() { return GpState{1, 0, 0, 0, 0, 0}; }
 
-// the entry at which the next boundary is crossed
+// the walk evaluates these rules (grandparents or a partitioner); without them only the size rule cuts files
+B200C_HD bool gp_rules_on(const GpCtx& c) { return c.n != 0 || c.np != 0; }
+// the next partition event, ~0 when there is none
+B200C_HD uint64_t gp_next_partition(const GpState& g, const GpCtx& c) { return g.part < c.np ? c.pev[g.part] : ~0ull; }
+// the entry at which the next boundary is crossed or the partitioner cuts, whichever comes first
 B200C_HD uint64_t gp_next_event(const GpState& g, const GpCtx& c) {
-  if (g.index >= c.n) return ~0ull;
-  return g.being_gap ? c.lo[g.index] : (c.next_same[g.index] ? c.eq[g.index] : c.hi[g.index]);
+  const uint64_t pe = gp_next_partition(g, c);
+  if (g.index >= c.n) return pe;
+  const uint64_t be = g.being_gap ? c.lo[g.index] : (c.next_same[g.index] ? c.eq[g.index] : c.hi[g.index]);
+  return be < pe ? be : pe;
 }
 // GetCurrentKeyGrandparentOverlappedBytes (:189-229) for the key of entry e
 B200C_HD uint64_t gp_overlap_at(const GpState& g, const GpCtx& c, uint64_t e) {
@@ -94,12 +108,15 @@ B200C_HD void gp_file_started(GpState& g, const GpCtx& c, uint64_t e) {
 // Every event seen here lies behind the open file's first entry: each file start was passed to gp_advance (the stream's first entry
 // before the walk, the cut returned here, the entry behind gp_size_cut's), and gp_next_event is always beyond the last entry
 // advanced to.  So the rules never stop in front of a file's first key, and no guard for that is needed.
+// A partition event ends the file whatever the other rules say; the boundary state has moved to that entry first (:247-253).
 B200C_HD uint64_t gp_block_cut(GpState& g, const GpCtx& c, uint64_t end, uint64_t n, uint64_t cur) {
   uint64_t ev;
   while ((ev = gp_next_event(g, c)) <= end && ev < n) {
     const uint64_t prev_overlapped = g.overlapped;
     const uint32_t crossed = gp_advance(g, c, ev);
-    if (gp_should_stop(g, c, crossed, prev_overlapped, cur)) {
+    const bool partition = ev == gp_next_partition(g, c);
+    if (partition) g.part++;
+    if (partition || gp_should_stop(g, c, crossed, prev_overlapped, cur)) {
       gp_file_started(g, c, ev);
       return ev;
     }
@@ -107,10 +124,11 @@ B200C_HD uint64_t gp_block_cut(GpState& g, const GpCtx& c, uint64_t end, uint64_
   return ~0ull;
 }
 // the size rule closed the file behind entry e - 1 (:277): ShouldStopBefore(e) moved the boundary state before the rule fired, and
-// entry e starts the next file
+// entry e starts the next file.  A partition event at e asks for the same cut (it is checked first, :264-269) and is used up by it.
 B200C_HD void gp_size_cut(GpState& g, const GpCtx& c, uint64_t e, uint64_t n) {
   if (e >= n) return;
   gp_advance(g, c, e);
+  if (gp_next_partition(g, c) == e) g.part++;
   gp_file_started(g, c, e);
 }
 

@@ -140,7 +140,7 @@ void launch_merge_sizes_fix(KeyCols merged, const unsigned long long* tile_state
 // Grandparent-aware output cutting (CompactionOutputs::ShouldStopBefore, compaction_outputs.cc:231-354).  The walk over the block
 // chain only needs to know at which merged ENTRY each boundary of a grandparent file is crossed, so the boundaries are turned
 // into entry ranks once (gp_rank_kernel) and the reference's key-driven state machine runs on ranks.
-struct GpCut {                 // an output file that was cut in front of `entry` by a grandparent rule
+struct GpCut {                 // an output file that was cut in front of `entry` by a grandparent rule or the partitioner
   uint64_t entry;
   uint64_t block_bytes;        // on-disk bytes of the (truncated) block that ends in front of it
 };
@@ -149,7 +149,7 @@ struct EncodeParams {
   uint32_t checksum, format_version, output_level;
   uint64_t max_output_file_size;
   GpCtx gp;
-  GpCut* gp_cuts;              // written by the stitch kernel (capacity 2 * gp.n + 2), replayed by the block-list kernel
+  GpCut* gp_cuts;              // written by the stitch kernel (capacity 2 * gp.n + 2 + gp.np), replayed by the block-list kernel
   uint32_t* gp_ncuts;
 };
 using GpKey = BoundKey;       // grandparent boundary key in column form
@@ -160,6 +160,11 @@ void launch_bloom_count(KeyCols m, uint64_t n, FileRec* files, const uint64_t* n
 // every filter block (8 u64 per full 1024-byte block; per file its first slot)
 void launch_bloom_build(const uint64_t* hashes, uint64_t n, const FileRec* files, uint32_t nfiles, uint32_t max_filter_bytes, uint32_t millibits, uint32_t cksum,
                         uint8_t* const* out_base, uint64_t* contrib, const uint64_t* contrib_off, cudaStream_t st);
+// fixed-prefix partitioner: the merged entries in front of which it cuts (gp_rules.h), ascending, into ev[0, cap); ev must hold ~0
+// and ticket / state (partition_event_tiles(m.n) words) zero beforehand.  More than cap events set kErrTooManyFiles.
+uint64_t partition_event_tiles(uint64_t n);
+void launch_partition_events(KeyCols m, uint32_t len, uint32_t cap, uint32_t* ticket, unsigned long long* state, uint64_t* ev, uint32_t* err,
+                             cudaStream_t st);
 void launch_gp_ranks(KeyCols m, const GpKey* smallest, const GpKey* largest, uint32_t n, uint64_t* lo, uint64_t* eq, uint64_t* hi,
                      cudaStream_t st);
 struct BlockRec {            // one output data block

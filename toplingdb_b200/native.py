@@ -39,7 +39,7 @@ class Params(C.Structure):
         ("range_start_user_key", C.c_char_p), ("range_start_len", C.c_uint32), ("has_range_start", C.c_uint32),
         ("range_end_user_key", C.c_char_p), ("range_end_len", C.c_uint32), ("has_range_end", C.c_uint32),
         ("paranoid_file_checks", C.c_uint32), ("bloom_millibits_per_key", C.c_uint32),
-        ("earliest_write_conflict_snapshot", C.c_uint64),
+        ("earliest_write_conflict_snapshot", C.c_uint64), ("sst_partitioner_prefix_len", C.c_uint32),
     ]
 
 
@@ -138,7 +138,8 @@ def block_checksums(kind, buffers, last_byte=0, device=0):
 class CompactionJob:
     """One compaction job = what CompactionExecutor::Execute receives (db/compaction/compaction_executor.h:160-178).
 
-    Keyword arguments are the b200c_params fields; `checksum` takes "xxh3" / "crc32c" / "none"."""
+    Keyword arguments are the b200c_params fields; `checksum` takes "xxh3" / "crc32c" / "none".  `sst_partitioner_prefix_len=N`
+    cuts the output files where the first N bytes of the user key change (SstPartitionerFixedPrefixFactory(N); 0 = none)."""
 
     def __init__(self, parent=None, **kw):
         L = lib()

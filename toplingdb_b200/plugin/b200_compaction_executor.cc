@@ -28,6 +28,7 @@
 #include "rocksdb/comparator.h"
 #include "rocksdb/env.h"
 #include "rocksdb/file_system.h"
+#include "rocksdb/sst_partitioner.h"
 #include "rocksdb/table.h"
 #include "table/block_based/filter_policy_internal.h"
 
@@ -68,6 +69,20 @@ int DeviceBloomMillibits(const Compaction* c, const BlockBasedTableOptions* t) {
   if (t->partition_filters || !t->whole_key_filtering || t->optimize_filters_for_memory || t->format_version < 5) return -1;
   if (c->mutable_cf_options()->prefix_extractor != nullptr) return -1;
   return static_cast<const BloomLikeFilterPolicy*>(fp)->GetMillibitsPerKey();
+}
+
+// Output partitioner of the column family (b200c_params::sst_partitioner_prefix_len): 0 = none; the prefix length of the stock
+// SstPartitionerFixedPrefixFactory, read through its registered option "length" (db/compaction/sst_partitioner.cc); < 0 = any
+// other partitioner, whose cuts the device cannot know: the job stays on the CPU.
+int64_t DevicePartitionerPrefixLen(const Compaction* c) {
+  const auto& f = c->immutable_options()->sst_partitioner_factory;
+  if (f == nullptr) return 0;
+  if (strcmp(f->Name(), SstPartitionerFixedPrefixFactory::kClassName()) != 0) return -1;
+  std::string v;
+  ConfigOptions co;
+  if (!f->GetOption(co, "length", &v).ok()) return -1;
+  const unsigned long long len = strtoull(v.c_str(), nullptr, 10);
+  return (int64_t)std::min<unsigned long long>(len, 0xffffffffull);  // >= 16 already means "the user key changed" on the device
 }
 
 // Output-file cut rules of CompactionOutputs::ShouldStopBefore (compaction_outputs.cc:231-354) that the device does NOT evaluate: the
@@ -236,6 +251,7 @@ class B200CompactionExecutor : public CompactionExecutor {
     bp.paranoid_file_checks = p.paranoid_file_checks;  // RunRemote cannot hash what it did not write (compaction_job.cc:1065-1068)
     bp.bloom_millibits_per_key = (uint32_t)std::max(0, DeviceBloomMillibits(c_, bbt));
     bp.earliest_write_conflict_snapshot = p.earliest_write_conflict_snapshot;
+    bp.sst_partitioner_prefix_len = (uint32_t)std::max<int64_t>(0, DevicePartitionerPrefixLen(c_));
     std::vector<uint64_t> snaps;
     if (p.existing_snapshots) snaps.assign(p.existing_snapshots->begin(), p.existing_snapshots->end());
     bp.snapshots = snaps.data();
@@ -632,7 +648,7 @@ static const char* WhyLocal(const Compaction* c) {
   if (io->compaction_filter_factory != nullptr && DeviceFilterOf(c) == B200C_FILTER_NONE) return "compaction filter the device does not implement";
   if (io->user_comparator != BytewiseComparator()) return "comparator other than the bytewise one (incl. user-defined timestamps)";
   if (c->output_compression() != kNoCompression) return "block compression";
-  if (io->sst_partitioner_factory != nullptr) return "sst partitioner";
+  if (DevicePartitionerPrefixLen(c) < 0) return "sst partitioner";
   if (io->allow_ingest_behind) return "allow_ingest_behind (no sequence-number zeroing, compaction_iterator.cc:1299-1304)";
   if (io->preclude_last_level_data_seconds > 0 || io->preserve_internal_time_seconds > 0)
     return "seqno-to-time preservation (preserve_time_min_seqno_, per-key placement)";
