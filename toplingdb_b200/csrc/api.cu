@@ -835,7 +835,7 @@ int encode_stage(b200c_job* j, KeyCols mcols, uint64_t n_out, uint32_t min_s1, u
     uint64_t data_bytes = 0;
     for (uint32_t f = 0; f < nfiles; f++) data_bytes += frs[f].data_size;
     j->kt_begin("encode.emit");
-    launch_encode_emit(mcols, ep, W, nblocks, out_base_d, data_bytes, err, j->sms, st);
+    launch_encode_emit(mcols, ep, W, nblocks, out_base_d, data_bytes, j->sms, st);
     j->kt_end();
     j->launches += 3;
     // The index blocks are written on the side stream beside the emit kernel (a file's index block lies behind its data and filter

@@ -1209,52 +1209,9 @@ __device__ __forceinline__ void store_bytes24(uint8_t* p, uint64_t S0, uint64_t 
   for (int k = 0; k < 8; k++)
     if ((uint32_t)(16 + k) < n) p[16 + k] = (uint8_t)(S2 >> (8 * k));
 }
-// n <= 64 value bytes: aligned word loads issued together, byte stores only for the unaligned head / tail of the
-// destination, 4-byte stores in between
-__device__ __forceinline__ void copy_value_small(uint8_t* dst, const uint8_t* src, uint32_t n) {
-  const uint32_t a = (uint32_t)((uintptr_t)src & 3);
-  const uint32_t* ws = reinterpret_cast<const uint32_t*>((uintptr_t)src - a);
-  const uint32_t nw = (a + n + 3) >> 2;  // <= 17
-  uint32_t w[18];
-#pragma unroll
-  for (int i = 0; i < 17; i++) w[i] = (uint32_t)i < nw ? __ldg(ws + i) : 0u;
-  w[17] = 0;
-  uint32_t head = (4 - (uint32_t)((uintptr_t)dst & 3)) & 3;
-  if (head > n) head = n;
-  {  // head bytes straight from the first words
-    const uint32_t v = __funnelshift_r(w[0], w[1], a * 8);
-    if (head > 0) dst[0] = (uint8_t)v;
-    if (head > 1) dst[1] = (uint8_t)(v >> 8);
-    if (head > 2) dst[2] = (uint8_t)(v >> 16);
-  }
-  const uint32_t t0 = a + head, bs = (t0 & 3) * 8;
-  const uint32_t nwords = (n - head) >> 2;
-  uint32_t* d32 = reinterpret_cast<uint32_t*>(dst + head);
-  uint32_t last;
-  if ((t0 >> 2) == 0) {
-#pragma unroll
-    for (int mI = 0; mI < 16; mI++)
-      if ((uint32_t)mI < nwords) d32[mI] = __funnelshift_r(w[mI], w[mI + 1], bs);
-    last = 0;
-  } else {
-#pragma unroll
-    for (int mI = 0; mI < 16; mI++)
-      if ((uint32_t)mI < nwords) d32[mI] = __funnelshift_r(w[mI + 1], w[mI + 2], bs);
-    last = 1;
-  }
-  const uint32_t done = head + 4 * nwords, rem = n - done;  // 0..3 tail bytes
-  if (rem) {
-    // tail word index = last + nwords (dynamic): fetch it again instead of indexing the register array dynamically
-    const uint32_t k = last + nwords;
-    const uint32_t lo = __ldg(ws + k), hi = (k + 1 < nw) ? __ldg(ws + k + 1) : 0u;
-    const uint32_t v = __funnelshift_r(lo, hi, bs);
-    dst[done] = (uint8_t)v;
-    if (rem > 1) dst[done + 1] = (uint8_t)(v >> 8);
-    if (rem > 2) dst[done + 2] = (uint8_t)(v >> 16);
-  }
-}
-// the store half of copy_value_small for a value whose aligned source words w[0..NW) are already in registers
-// (w[NW] must be 0); a = source misalignment, n <= 4 * (NW - 1) bytes
+// n value bytes whose aligned source words w[0..NW) are already in registers (w[NW] must be 0) to an arbitrarily aligned
+// shared-memory address: byte stores only for the unaligned head / tail of the destination, 4-byte stores in between;
+// a = source misalignment, n <= 4 * (NW - 1) bytes
 template <int NW>
 __device__ __forceinline__ void store_value_words(uint8_t* dst, const uint32_t* w, uint32_t a, uint32_t n) {
   if (n == 0) return;
@@ -1291,6 +1248,17 @@ __device__ __forceinline__ void store_value_words(uint8_t* dst, const uint32_t* 
     if (rem > 1) dst[done + 1] = (uint8_t)(tailv >> 8);
     if (rem > 2) dst[done + 2] = (uint8_t)(tailv >> 16);
   }
+}
+// n (1..64) value bytes: the 17 aligned words that cover them at any phase are loaded together, then stored as above
+__device__ __forceinline__ void copy_value_small(uint8_t* dst, const uint8_t* src, uint32_t n) {
+  const uint32_t a = (uint32_t)((uintptr_t)src & 3);
+  const uint32_t* ws = reinterpret_cast<const uint32_t*>((uintptr_t)src - a);
+  const uint32_t nw = (a + n + 3) >> 2;  // <= 17
+  uint32_t w[18];
+#pragma unroll
+  for (int i = 0; i < 17; i++) w[i] = (uint32_t)i < nw ? __ldg(ws + i) : 0u;
+  w[17] = 0;
+  store_value_words<17>(dst, w, a, n);
 }
 constexpr int kEmitPerLane = 3;
 constexpr int kEmitMaxEntries = 32 * kEmitPerLane;  // 96 entries per block on the fast path
@@ -1360,6 +1328,18 @@ __device__ __forceinline__ void emit_copy_long_value(uint8_t* dp, const uint8_t*
     }
   }
 }
+// Warp-level: the values longer than 64 bytes among the lanes' (value length vs, image offset voff), one after another, each
+// copied by the whole warp; vref_of(sl) gives lane sl's value reference to every lane.
+template <class VrefOf>
+__device__ __forceinline__ void emit_long_values(uint8_t* img, uint32_t vs, uint32_t voff, VrefOf vref_of, unsigned lane) {
+  unsigned big = __ballot_sync(0xffffffffu, vs > 64);
+  while (big) {
+    const int sl = __ffs(big) - 1;
+    big &= big - 1;
+    const uint32_t vl = __shfl_sync(0xffffffffu, vs, sl), vo = __shfl_sync(0xffffffffu, voff, sl);
+    emit_copy_long_value(img + vo, (const uint8_t*)(uintptr_t)vref_of(sl), vl, lane);
+  }
+}
 // Warp-level: restart count footer, checksum trailer, then the image (built at gdst's 16-byte phase `shift`) leaves as head bytes,
 // ONE bulk copy (TMA) of everything between the first and the last 16-byte boundary, and tail bytes
 __device__ __forceinline__ void emit_block_finish(uint8_t* img, uint8_t* gdst, uint32_t shift, uint32_t body, uint32_t nrest, uint32_t cksum,
@@ -1426,13 +1406,7 @@ __device__ __noinline__ void emit_block_warp(KeyCols m, const uint8_t* eshared, 
       if (vs && vs <= 64) copy_value_small(img + voff, (const uint8_t*)(uintptr_t)vref, vs);
     }
     // values longer than 64 bytes: the warp copies each of them with all lanes
-    unsigned big = __ballot_sync(0xffffffffu, vs > 64);
-    while (big) {
-      const int sl = __ffs(big) - 1;
-      big &= big - 1;
-      const uint32_t vl = __shfl_sync(0xffffffffu, vs, sl), vo = __shfl_sync(0xffffffffu, voff, sl);
-      emit_copy_long_value(img + vo, (const uint8_t*)(uintptr_t)__shfl_sync(0xffffffffu, vref, sl), vl, lane);
-    }
+    emit_long_values(img, vs, voff, [&](int sl) { return __shfl_sync(0xffffffffu, vref, sl); }, lane);
   }
   if (staged) {
     emit_block_finish(img, gdst, shift, (uint32_t)body, nrest, cksum, xtab, lane);
@@ -1444,6 +1418,88 @@ __device__ __noinline__ void emit_block_warp(KeyCols m, const uint8_t* eshared, 
   const uint32_t ck = block_checksum_warp(cksum, img, payload, 0);
   __syncwarp();  // the checksum's 8-byte loads may touch the trailer bytes written next
   if (lane == 0) put_block_trailer(img + payload, ck);
+}
+// ---- the fast path's steps, shared by both emit kernels (one warp per block of at most kEmitMaxEntries entries, lane l owning
+// entries [3l, 3l + 3)).  The kernels differ only in where the columns come from -- the staged kernel reads a shared-memory stage,
+// the long-entry kernel loads from global memory -- so the steps take the lane's columns as accessors of the entry index i.
+constexpr int kEmitShortWords = 9;  // aligned words covering a value of <= 32 bytes at any 4-byte phase
+// The fit rule: the block's payload (body, restart array, restart count), its trailer, 32 bytes and the image's 16-byte phase fit
+// the warp's image slot.  A block that does not fit goes to emit_block_warp.
+__device__ __forceinline__ bool emit_block_fits(uint64_t body, uint32_t nrest, uint32_t slot_bytes) {
+  return body + 4ull * nrest + 4 + 5 + 32 + 16 <= slot_bytes;
+}
+// Lane-level size pass: sz / pk / vs of the lane's entries (0 beyond the block's E entries); returns the lane's total
+template <class MetaOf, class EshOf>
+__device__ __forceinline__ uint32_t emit_lane_sizes(uint32_t E, uint32_t R, uint32_t rmask, unsigned lane, MetaOf meta_of, EshOf esh_of,
+                                                    uint32_t (&sz)[kEmitPerLane], uint32_t (&pk)[kEmitPerLane], uint32_t (&vs)[kEmitPerLane]) {
+  uint32_t tsum = 0;
+#pragma unroll
+  for (int i = 0; i < kEmitPerLane; i++) {
+    const uint32_t x = lane * kEmitPerLane + i;
+    sz[i] = pk[i] = vs[i] = 0;
+    if (x < E) {
+      sz[i] = entry_pack(meta_of(i), esh_of(i), x, R, rmask, &pk[i], &vs[i]);
+      tsum += sz[i];
+    }
+  }
+  return tsum;
+}
+// Lane-level: the image offsets of the lane's entries from the start of its run (the exclusive warp scan of the lane totals)
+__device__ __forceinline__ void emit_lane_offsets(uint32_t run, const uint32_t (&sz)[kEmitPerLane], uint32_t (&off)[kEmitPerLane]) {
+#pragma unroll
+  for (int i = 0; i < kEmitPerLane; i++) {
+    off[i] = run;
+    run += sz[i];
+  }
+}
+// Lane-level: header + key suffix of the lane's entries; voff = image offset of each entry's value bytes
+template <class PfxOf, class TrOf>
+__device__ __forceinline__ void emit_lane_keys(uint8_t* img, uint32_t E, uint32_t body, uint32_t R, uint32_t rmask, unsigned lane,
+                                               const uint32_t (&off)[kEmitPerLane], const uint32_t (&pk)[kEmitPerLane],
+                                               const uint32_t (&vs)[kEmitPerLane], PfxOf pfx_of, TrOf tr_of, uint32_t (&voff)[kEmitPerLane]) {
+#pragma unroll
+  for (int i = 0; i < kEmitPerLane; i++) {
+    const uint32_t x = lane * kEmitPerLane + i;
+    voff[i] = 0;
+    if (x < E) {
+      const ulonglong2 pp = pfx_of(i);
+      voff[i] = emit_entry_key(img, off[i], pk[i], vs[i], pp.x, pp.y, tr_of(i), x, body, R, rmask);
+    }
+  }
+}
+__device__ __forceinline__ bool emit_all_short(const uint32_t (&vs)[kEmitPerLane]) {
+  bool all_short = true;
+#pragma unroll
+  for (int i = 0; i < kEmitPerLane; i++) all_short = all_short && vs[i] <= 32;
+  return all_short;
+}
+// Lane-level: the values of a group whose values are all <= 32 bytes, from words the kernel has loaded: words(i, w) puts entry i's
+// aligned words in w[0..kEmitShortWords) (w[kEmitShortWords] = 0) and returns the value's 4-byte phase
+template <class Words>
+__device__ __forceinline__ void emit_lane_short_values(uint8_t* img, const uint32_t (&voff)[kEmitPerLane], const uint32_t (&vs)[kEmitPerLane],
+                                                       Words words) {
+#pragma unroll
+  for (int i = 0; i < kEmitPerLane; i++) {
+    if (!vs[i]) continue;
+    uint32_t w[12];
+    const uint32_t a = words(i, w);
+    store_value_words<kEmitShortWords>(img + voff[i], w, a, vs[i]);
+  }
+}
+// Lane-level: the values of 1..64 bytes of a group that is not all short, each copied by its lane
+template <class VrefOf>
+__device__ __forceinline__ void emit_lane_copy_values(uint8_t* img, const uint32_t (&voff)[kEmitPerLane], const uint32_t (&vs)[kEmitPerLane],
+                                                      VrefOf vref_of) {
+#pragma unroll
+  for (int i = 0; i < kEmitPerLane; i++)
+    if (vs[i] && vs[i] <= 64) copy_value_small(img + voff[i], (const uint8_t*)(uintptr_t)vref_of(i), vs[i]);
+}
+// Warp-level: the values longer than 64 bytes of the lanes' groups, one after another, each copied by the whole warp
+template <class VrefOf>
+__device__ __forceinline__ void emit_group_long_values(uint8_t* img, const uint32_t (&voff)[kEmitPerLane], const uint32_t (&vs)[kEmitPerLane],
+                                                       VrefOf vref_of, unsigned lane) {
+#pragma unroll
+  for (int i = 0; i < kEmitPerLane; i++) emit_long_values(img, vs[i], voff[i], [&](int sl) { return vref_of(sl, i); }, lane);
 }
 constexpr int kEmitCtasPerSm = 3;                   // 12 warps per SM (with kEmitWarps = 4): room for 168 registers, no spills
 // A column stage holds one block's entries of every column, copied by TMA as the 16-byte-aligned cover of the entry range (the cover
@@ -1483,7 +1539,7 @@ __device__ __forceinline__ void emit_stage_fill(const KeyCols& m, const EncodeWo
 // or larger than the image slot take emit_block_warp (no stage: it reads the columns from global memory).
 __global__ void __launch_bounds__(kEmitWarps * 32, kEmitCtasPerSm)
 encode_emit_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t nblocks, uint8_t* const* __restrict__ out_base,
-                   uint32_t slot_bytes, uint32_t* __restrict__ err) {
+                   uint32_t slot_bytes) {
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ XxhLaneTab s_xtab;
   __shared__ __align__(8) uint64_t s_bar[kEmitWarps][2];
@@ -1546,17 +1602,10 @@ encode_emit_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t nblocks, 
     if (!fallback) {
       mbar_wait(bar0 + 8 * s, (parity >> s) & 1);
       parity ^= 1u << s;
-#pragma unroll
-      for (int i = 0; i < kEmitPerLane; i++) {
-        const uint32_t x = lane * kEmitPerLane + i;
-        sz[i] = pk[i] = vs[i] = 0;
-        if (x < E) {
-          sz[i] = entry_pack(c_meta[x], c_esh[x], x, R, rmask, &pk[i], &vs[i]);
-          tsum += sz[i];
-        }
-      }
+      const uint32_t x0 = lane * kEmitPerLane;
+      tsum = emit_lane_sizes(E, R, rmask, lane, [&](int i) { return c_meta[x0 + i]; }, [&](int i) { return c_esh[x0 + i]; }, sz, pk, vs);
       inc = warp_incl_scan64(tsum);
-      fallback = __shfl_sync(0xffffffffu, inc, 31) + 4ull * nrest + 4 + 5 + 32 + 16 > slot_bytes;
+      fallback = !emit_block_fits(__shfl_sync(0xffffffffu, inc, 31), nrest, slot_bytes);
     }
     if (fallback) {
       load_next();
@@ -1567,22 +1616,12 @@ encode_emit_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t nblocks, 
     }
     const uint32_t body = (uint32_t)__shfl_sync(0xffffffffu, inc, 31);
     uint32_t off[kEmitPerLane];
-    {
-      uint32_t run = (uint32_t)(inc - tsum);
-#pragma unroll
-      for (int i = 0; i < kEmitPerLane; i++) {
-        off[i] = run;
-        run += sz[i];
-      }
-    }
+    emit_lane_offsets((uint32_t)(inc - tsum), sz, off);
     // ---- value bytes of all the lane's entries (when every value is short) leave first; the key bytes are written meanwhile.
     // A value of <= 32 bytes lies in at most three aligned 16-byte chunks: three vector loads instead of nine word loads (the
     // lanes' values are scattered, so every load instruction touches one cache line per lane).  Value references are read from
     // the stage where they are used, so that no register holds them across the key work.
-    constexpr int kNW = 9;  // aligned words covering a value of <= 32 bytes at any 4-byte phase
-    bool all_short = true;
-#pragma unroll
-    for (int i = 0; i < kEmitPerLane; i++) all_short = all_short && vs[i] <= 32;
+    const bool all_short = emit_all_short(vs);
     uint4 vc[kEmitPerLane][3];
     if (all_short) {
 #pragma unroll
@@ -1597,25 +1636,18 @@ encode_emit_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t nblocks, 
     }
     if (lane == 0) bulk_wait_read0();  // the previous block's bulk store has finished reading the slot
     __syncwarp();
+    const uint32_t x0 = lane * kEmitPerLane;
     uint32_t voff[kEmitPerLane];  // image offset of the value bytes
-#pragma unroll
-    for (int i = 0; i < kEmitPerLane; i++) {
-      const uint32_t x = lane * kEmitPerLane + i;
-      voff[i] = 0;
-      if (x < E) {
-        const ulonglong2 pp = c_pfx[x];
-        voff[i] = emit_entry_key(img, off[i], pk[i], vs[i], pp.x, pp.y, c_tr[x], x, body, R, rmask);
-      }
-    }
+    emit_lane_keys(img, E, body, R, rmask, lane, off, pk, vs, [&](int i) { return c_pfx[x0 + i]; }, [&](int i) { return c_tr[x0 + i]; }, voff);
     if (all_short) {
+      emit_lane_short_values(img, voff, vs, [&](int i, uint32_t(&w)[12]) {
+        const uint32_t a = (uint32_t)(c_vref[x0 + i] & 15);
+        const uint32_t t[12] = {vc[i][0].x, vc[i][0].y, vc[i][0].z, vc[i][0].w, vc[i][1].x, vc[i][1].y,
+                                vc[i][1].z, vc[i][1].w, vc[i][2].x, vc[i][2].y, vc[i][2].z, vc[i][2].w};
 #pragma unroll
-      for (int i = 0; i < kEmitPerLane; i++) {
-        if (!vs[i]) continue;
-        const uint32_t a = (uint32_t)(c_vref[lane * kEmitPerLane + i] & 15);
-        uint32_t w[12] = {vc[i][0].x, vc[i][0].y, vc[i][0].z, vc[i][0].w, vc[i][1].x, vc[i][1].y,
-                          vc[i][1].z, vc[i][1].w, vc[i][2].x, vc[i][2].y, vc[i][2].z, vc[i][2].w};
-        // drop the a / 4 words in front of the value: w[0..kNW) then covers it at the 4-byte phase a & 3 (a & 3 + 32 bytes end
-        // inside w[8]), and w[kNW] = 0 as store_value_words expects
+        for (int k = 0; k < 12; k++) w[k] = t[k];
+        // drop the a / 4 words in front of the value: w[0..9) then covers it at the 4-byte phase a & 3 (a & 3 + 32 bytes end
+        // inside w[8]), and w[9] = 0 as store_value_words expects
         if (a & 8) {
 #pragma unroll
           for (int k = 0; k < 10; k++) w[k] = w[k + 2];
@@ -1624,31 +1656,17 @@ encode_emit_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t nblocks, 
 #pragma unroll
           for (int k = 0; k < 11; k++) w[k] = w[k + 1];
         }
-        w[kNW] = 0;
-        store_value_words<kNW>(img + voff[i], w, a & 3, vs[i]);
-      }
+        w[kEmitShortWords] = 0;
+        return a & 3;
+      });
     } else {
-#pragma unroll
-      for (int i = 0; i < kEmitPerLane; i++)
-        if (vs[i] && vs[i] <= 64) copy_value_small(img + voff[i], (const uint8_t*)(uintptr_t)c_vref[lane * kEmitPerLane + i], vs[i]);
+      emit_lane_copy_values(img, voff, vs, [&](int i) { return c_vref[x0 + i]; });
     }
-    // values longer than 64 bytes: the warp copies each of them with all lanes
-#pragma unroll
-    for (int i = 0; i < kEmitPerLane; i++) {
-      unsigned big = __ballot_sync(0xffffffffu, vs[i] > 64);
-      while (big) {
-        const int sl = __ffs(big) - 1;
-        big &= big - 1;
-        const uint32_t vl = __shfl_sync(0xffffffffu, vs[i], sl);
-        const uint32_t vo = __shfl_sync(0xffffffffu, voff[i], sl);
-        emit_copy_long_value(img + vo, (const uint8_t*)(uintptr_t)c_vref[sl * kEmitPerLane + i], vl, lane);
-      }
-    }
+    emit_group_long_values(img, voff, vs, [&](int sl, int i) { return c_vref[sl * kEmitPerLane + i]; }, lane);
     load_next();
     emit_block_finish(img, gdst, shift, body, nrest, ep.checksum, xtab, lane);
   }
   if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // no bulk store may outlive the CTA's shared memory
-  (void)err;
 }
 
 constexpr int kEmitLongWarps = 8, kEmitLongCtasPerSm = 4;  // 32 warps per SM, 64 registers each
@@ -1660,7 +1678,7 @@ constexpr int kEmitLongWarps = 8, kEmitLongCtasPerSm = 4;  // 32 warps per SM, 6
 // three DRAM round trips.  Blocks with more than 96 entries or larger than the image slot take emit_block_warp.
 __global__ void __launch_bounds__(kEmitLongWarps * 32, kEmitLongCtasPerSm)
 encode_emit_long_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t nblocks, uint8_t* const* __restrict__ out_base,
-                   uint32_t slot_bytes, uint32_t* __restrict__ err) {
+                        uint32_t slot_bytes) {
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ XxhLaneTab s_xtab;
   const unsigned lane = threadIdx.x & 31, w = threadIdx.x >> 5;
@@ -1701,17 +1719,9 @@ encode_emit_long_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t nblo
           vrf[i] = m.vref[e0 + x];
         }
       }
-#pragma unroll
-      for (int i = 0; i < kEmitPerLane; i++) {
-        const uint32_t x = lane * kEmitPerLane + i;
-        sz[i] = pk[i] = vs[i] = 0;
-        if (x < E) {
-          sz[i] = entry_pack(mtv[i], shv[i], x, R, rmask, &pk[i], &vs[i]);
-          tsum += sz[i];
-        }
-      }
+      tsum = emit_lane_sizes(E, R, rmask, lane, [&](int i) { return mtv[i]; }, [&](int i) { return shv[i]; }, sz, pk, vs);
       inc = warp_incl_scan64(tsum);
-      fallback = __shfl_sync(0xffffffffu, inc, 31) + 4ull * nrest + 4 + 5 + 32 + 16 > slot_bytes;
+      fallback = !emit_block_fits(__shfl_sync(0xffffffffu, inc, 31), nrest, slot_bytes);
     }
     if (lane == 0) bulk_wait_read0();  // the previous block's bulk store has finished reading the slot (the loads above overlapped it)
     __syncwarp();
@@ -1721,14 +1731,7 @@ encode_emit_long_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t nblo
     }
     const uint32_t body = (uint32_t)__shfl_sync(0xffffffffu, inc, 31);
     uint32_t off[kEmitPerLane];
-    {
-      uint32_t run = (uint32_t)(inc - tsum);
-#pragma unroll
-      for (int i = 0; i < kEmitPerLane; i++) {
-        off[i] = run;
-        run += sz[i];
-      }
-    }
+    emit_lane_offsets((uint32_t)(inc - tsum), sz, off);
     // ---- pass 2: key columns of all the lane's entries, then all value words (when every value is short)
     uint32_t voff[kEmitPerLane];  // image offset of the value bytes
     {
@@ -1744,56 +1747,31 @@ encode_emit_long_kernel(KeyCols m, EncodeParams ep, EncodeWork wk, uint64_t nblo
           trv[i] = m.tr[e0 + x];
         }
       }
+      emit_lane_keys(img, E, body, R, rmask, lane, off, pk, vs, [&](int i) { return ppv[i]; }, [&](int i) { return trv[i]; }, voff);
+    }
+    if (emit_all_short(vs)) {
+      uint32_t vw[kEmitPerLane][kEmitShortWords + 1];
 #pragma unroll
       for (int i = 0; i < kEmitPerLane; i++) {
-        const uint32_t x = lane * kEmitPerLane + i;
-        voff[i] = 0;
-        if (x < E) {
-          voff[i] = emit_entry_key(img, off[i], pk[i], vs[i], ppv[i].x, ppv[i].y, trv[i], x, body, R, rmask);
-        }
+        const uint32_t a = (uint32_t)(vrf[i] & 3);
+        const uint32_t* wsrc = reinterpret_cast<const uint32_t*>((uintptr_t)vrf[i] - a);
+        const uint32_t nw = vs[i] ? (a + vs[i] + 3) >> 2 : 0;
+#pragma unroll
+        for (int k = 0; k < kEmitShortWords; k++) vw[i][k] = (uint32_t)k < nw ? __ldg(wsrc + k) : 0u;
+        vw[i][kEmitShortWords] = 0;
       }
+      emit_lane_short_values(img, voff, vs, [&](int i, uint32_t(&w)[12]) {
+#pragma unroll
+        for (int k = 0; k <= kEmitShortWords; k++) w[k] = vw[i][k];
+        return (uint32_t)(vrf[i] & 3);
+      });
+    } else {
+      emit_lane_copy_values(img, voff, vs, [&](int i) { return vrf[i]; });
     }
-    {
-      constexpr int kNW = 9;  // aligned words covering a value of <= 32 bytes at any alignment
-      bool all_short = true;
-#pragma unroll
-      for (int i = 0; i < kEmitPerLane; i++) all_short = all_short && vs[i] <= 32;
-      if (all_short) {
-        uint32_t vw[kEmitPerLane][kNW + 1];
-#pragma unroll
-        for (int i = 0; i < kEmitPerLane; i++) {
-          const uint32_t a = (uint32_t)(vrf[i] & 3);
-          const uint32_t* wsrc = reinterpret_cast<const uint32_t*>((uintptr_t)vrf[i] - a);
-          const uint32_t nw = vs[i] ? (a + vs[i] + 3) >> 2 : 0;
-#pragma unroll
-          for (int k = 0; k < kNW; k++) vw[i][k] = (uint32_t)k < nw ? __ldg(wsrc + k) : 0u;
-          vw[i][kNW] = 0;
-        }
-#pragma unroll
-        for (int i = 0; i < kEmitPerLane; i++) store_value_words<kNW>(img + voff[i], vw[i], (uint32_t)(vrf[i] & 3), vs[i]);
-      } else {
-#pragma unroll
-        for (int i = 0; i < kEmitPerLane; i++)
-          if (vs[i] && vs[i] <= 64) copy_value_small(img + voff[i], (const uint8_t*)(uintptr_t)vrf[i], vs[i]);
-      }
-    }
-    // values longer than 64 bytes: the warp copies each of them with all lanes
-#pragma unroll
-    for (int i = 0; i < kEmitPerLane; i++) {
-      unsigned big = __ballot_sync(0xffffffffu, vs[i] > 64);
-      while (big) {
-        const int sl = __ffs(big) - 1;
-        big &= big - 1;
-        const uint32_t vl = __shfl_sync(0xffffffffu, vs[i], sl);
-        const uint32_t vo = __shfl_sync(0xffffffffu, voff[i], sl);
-        const uint64_t vrr = __shfl_sync(0xffffffffu, vrf[i], sl);
-        emit_copy_long_value(img + vo, (const uint8_t*)(uintptr_t)vrr, vl, lane);
-      }
-    }
+    emit_group_long_values(img, voff, vs, [&](int sl, int i) { return __shfl_sync(0xffffffffu, vrf[i], sl); }, lane);
     emit_block_finish(img, gdst, shift, body, nrest, ep.checksum, xtab, lane);
   }
   if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // no bulk store may outlive the CTA's shared memory
-  (void)err;
 }
 
 // ------------------------------------------------------------------------------------------------ index block
@@ -2351,7 +2329,7 @@ uint32_t encode_emit_slice(uint32_t block_size) {
 }
 static_assert(kEmitWarps * (24 * 1024 + 2 * kStageBytes) <= kEmitMaxSmem, "the largest slots and their column stages fit one CTA");
 void launch_encode_emit(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nblocks, uint8_t* const* out_base, uint64_t data_bytes,
-                        uint32_t* err, int sms, cudaStream_t st) {
+                        int sms, cudaStream_t st) {
   if (nblocks == 0) return;
   static PerDeviceFlag attr;
   const uint64_t dev_bit = attr.bit_of_current_device();
@@ -2379,8 +2357,8 @@ void launch_encode_emit(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nbloc
   // queue behind the last emit CTA.
   const uint64_t cap = (uint64_t)sms * per_sm;
   const unsigned grid = (unsigned)(want < cap ? want : cap);
-  if (long_entries) encode_emit_long_kernel<<<grid, warps * 32, smem, st>>>(m, ep, w, nblocks, out_base, slot, err);
-  else encode_emit_kernel<<<grid, warps * 32, smem, st>>>(m, ep, w, nblocks, out_base, slot, err);
+  if (long_entries) encode_emit_long_kernel<<<grid, warps * 32, smem, st>>>(m, ep, w, nblocks, out_base, slot);
+  else encode_emit_kernel<<<grid, warps * 32, smem, st>>>(m, ep, w, nblocks, out_base, slot);
 }
 static unsigned index_grid(uint64_t nblocks, int sms) {
   const uint64_t g = (nblocks + 255) / 256;

@@ -248,7 +248,7 @@ void launch_encode_filestats(KeyCols m, EncodeWork w, uint32_t nfiles, cudaStrea
 uint32_t encode_emit_slice(uint32_t block_size);
 // out_base[f] = device address where file f's image starts; data_bytes = all data blocks incl. trailers (with m.n: selects the kernel)
 void launch_encode_emit(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nblocks, uint8_t* const* out_base, uint64_t data_bytes,
-                        uint32_t* err, int sms, cudaStream_t st);
+                        int sms, cudaStream_t st);
 // index blocks in two steps: separators, entry sizes and their scan (what the file sizes need), then the entries, restart arrays and
 // trailers written into the images
 void launch_encode_index_size(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nblocks, int sms, cudaStream_t st, uint64_t* launches);
