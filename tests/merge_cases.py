@@ -36,7 +36,7 @@ SNAP_CACHE = _constant("merge.cu", "kSnapCache")
 MAX_USER_KEY = 16
 SEQ_HI = 1 << 22
 TTL, NOW = 1000, 1_000_000
-DELETION, VALUE = 0, 1
+DELETION, VALUE, SINGLE_DELETION = 0, 1, 7
 # what the compaction iterator and the whole job count alike.  num_input_records is not among them: the job sums the input files' entry
 # counts (UpdateCompactionInputStatsHelper, compaction_job.cc:2383-2396), the iterator counts the entries it stepped on.
 STAGE_STAT_KEYS = tuple(k for k in H.STAT_KEYS if k != "num_input_records") + ("num_record_drop_user",)
@@ -95,11 +95,13 @@ class _Stream:
         return struct.pack(">QQ", i >> 8, ((i & 255) << 56) | ((i * 0x9E3779B97F4A7C15) & ((1 << 56) - 1)))
 
     def add(self, ukey, versions):
-        """versions: [(seq, type, value)], any order; every version goes to a random run"""
+        """versions: [(seq, type, value)] or [(seq, type, value, run)], any order; a version without a run goes to a random one.
+        Tombstones (Deletion, SingleDeletion) are stored without a value."""
         assert len(ukey) <= MAX_USER_KEY and (not self.keys or self.keys[-1][0] < ukey)
         vs = sorted(versions, key=lambda v: -v[0])
-        assert len({v[0] for v in vs}) == len(vs)
-        self.keys.append((ukey, [(s, t, b"" if t == DELETION else v, self.rnd.randrange(self.nruns)) for s, t, v in vs]))
+        assert len({v[0] for v in vs}) == len(vs) and all(v[1] in (DELETION, VALUE, SINGLE_DELETION) for v in vs)
+        self.keys.append((ukey, [(v[0], v[1], v[2] if v[1] == VALUE else b"", v[3] if len(v) > 3 else self.rnd.randrange(self.nruns))
+                                 for v in vs]))
         self.pos += len(vs)
 
     def ordinary(self, n, max_versions=3):

@@ -29,6 +29,7 @@ namespace b200c {
 constexpr int kMT = kMergeTile;
 constexpr int kMThreads = 256;
 constexpr int kMV = kMT / kMThreads;  // 8 merged entries per thread
+constexpr uint32_t kPartGroupedMaxRuns = 16;  // runs that merge_partition_grouped_kernel takes (a group of at least 2 lanes each)
 
 __device__ __forceinline__ Key load_key(const KeyCols& c, uint64_t i) {
   Key k;
@@ -509,8 +510,10 @@ __device__ __noinline__ void sd_walk_tile(TileSmem& s, const KeyCols& in, const 
     bool head = true;
     if (o > 0) {
       head = !same_ukey(skey(s, s.idx[PH(o - 1)]), k0);
-    } else if (s.has_pred && same_ukey(s.pred, k0)) {
-      atomicOr(err, (uint32_t)kErrInternal);  // the partition keeps keys inside one tile in this mode
+    } else if (s.has_pred && same_ukey(s.pred, k0) && k <= kPartGroupedMaxRuns) {
+      // the grouped partition keeps keys inside one tile in this mode; with more runs merge_partition_kernel leaves the cuts where they
+      // fall and has already refused the job (kErrGroupTooLong): that refusal is the job's answer, not an internal error
+      atomicOr(err, (uint32_t)kErrInternal);
     }
     if (!head) continue;
     GroupVersion gv[kMaxGroup];
@@ -1160,7 +1163,7 @@ void launch_run_bounds(KeyCols in, const uint64_t* file_start, const uint32_t* r
 void launch_merge_partition(KeyCols in, RunBounds runs, uint32_t nruns, uint64_t n_total, uint64_t ntiles,
                             uint64_t* splits, uint32_t* err, int sms, cudaStream_t st) {
   unsigned warps = (unsigned)(ntiles + 1);
-  if (nruns <= 16) {
+  if (nruns <= kPartGroupedMaxRuns) {
     uint32_t kp2 = 2;  // at most 16 lanes per run
     while (kp2 < nruns) kp2 <<= 1;
     uint32_t gshift = 0;
