@@ -1,5 +1,5 @@
-"""Jobs for what the encoder writes behind the data blocks of every output file: the index block (encode_index_sep_kernel,
-encode_index_size_kernel, encode_index_write_kernel in csrc/encode.cu), the full Bloom filter block (bloom_count_kernel,
+"""Jobs for what the encoder writes behind the data blocks of every output file: the index block (index_entry and
+shortest_separator in encode_index_size_kernel, then encode_index_write_kernel in csrc/encode.cu), the full Bloom filter block (bloom_count_kernel,
 bloom_layout_kernel, bloom_slices_kernel) and the checksums of both (file_block_contrib_kernel, file_block_trailer_kernel over
 xxh3_64_warp_t's precomputed-block path in csrc/common.cuh).
 

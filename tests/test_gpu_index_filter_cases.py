@@ -1,8 +1,11 @@
 """The index and filter jobs (tests/index_filter_cases.py) through the C ABI against the CPU oracle: output files, statistics and file
 metadata, a failure naming the region of the first differing byte (gpu_harness.describe_first_difference); a subset with
 device-resident inputs; a separator job and a two-slice filter through b200c_job_encode_kv (the B200TableBuilder path) against the
-oracle's table builder; exactly kMaxOutFiles output files, and one more refused with ERR_NOT_SUPPORTED.  The handles_* jobs hold about
+oracle's table builder; the launches the XXH3 checksums of the index and filter blocks add; exactly kMaxOutFiles output files, and
+one more refused with ERR_NOT_SUPPORTED.  The handles_* jobs hold about
 400 MB of values each and dominate the runtime."""
+import copy
+
 import pytest
 
 import helpers as H
@@ -60,6 +63,20 @@ def test_table_builder_path_matches_the_oracle_builder(name):
     finally:
         job.close()
     _same_files(name, files, [want])
+
+
+@pytest.mark.parametrize("name, blocks", [("filter_phases", 2), ("sep_v5_xxh3", 1)])
+def test_xxh3_adds_one_contribution_launch_per_checksummed_block(name, blocks):
+    """file_block_contrib_kernel runs only for XXH3: once over the index blocks and, with a filter policy, once over the filter blocks"""
+    from gpu_harness import run_product
+    p, inputs = C.build(name)
+    launches = {}
+    for ck in ("xxh3", "crc32c"):
+        q = copy.copy(p)
+        q.checksum = ck
+        launches[ck] = run_product(q, inputs)[2].kernel_launches
+    print(f"{name}: kernel launches {launches}")
+    assert launches["xxh3"] - launches["crc32c"] == blocks, launches
 
 
 def test_one_file_more_than_the_limit_is_refused():

@@ -17,6 +17,7 @@ ENCODE = open(os.path.join(C.plan_cases._CSRC, "encode.cu")).read()
 COMMON = open(os.path.join(C.plan_cases._CSRC, "common.cuh")).read()
 assert "if (d < nul - 1 || (uint32_t)s[d] + 1 < (uint32_t)l[d]) {" in ENCODE
 assert "sep = KeyRec{hi, lo, (kMaxSeq << 8) | 0x16, tn, 1};" in ENCODE
+assert "p = first_nonzero_byte(~hi & a.x & ~b.x, ~lo & a.y & ~b.y);" in ENCODE and "if (p == 16) return false;  // all 0xff" in ENCODE
 assert "const uint64_t nb_blocks = (len - 1) / 1024;" in COMMON and "for (; n + 8 <= nb_blocks; n += 8) {" in COMMON
 assert "if (len <= 240) return xxh3_64_short(in, (uint32_t)len);" in COMMON
 SEEK_TRAILER = struct.pack("<Q", (H.MAX_SEQ << 8) | 0x16)  # kMaxSequenceNumber, kValueTypeForSeek

@@ -16,7 +16,7 @@ GROUP = {  # kernel -> bench.py kernel group
     "merge_partition_kernel": "merge.partition", "merge_tiles_kernel": "merge.tiles", "merge_sizes_fix_kernel": "merge.sizes_fix",
     "encode_tables_kernel": "encode.tables", "encode_stitch_kernel": "~encode.stitch", "encode_tilestate_kernel": "encode.tilestate",
     "encode_blocklist_kernel": "encode.blocklist", "encode_emit_kernel": "encode.emit", "encode_filestats_kernel": "~encode.filestats+index",
-    "encode_index_sep_kernel": "~encode.filestats+index", "encode_index_size_kernel": "~encode.filestats+index",
+    "encode_index_size_kernel": "~encode.filestats+index",
     "encode_index_write_kernel": "~encode.filestats+index", "file_block_contrib_kernel": "~encode.filestats+index",
     "file_block_trailer_kernel": "~encode.filestats+index", "scan_tile_sums": "~encode.filestats+index", "scan_of_sums": "~encode.filestats+index",
     "scan_downsweep": "~encode.filestats+index", "run_bounds_kernel": "merge.partition",

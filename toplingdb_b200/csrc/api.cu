@@ -253,10 +253,10 @@ struct b200c_job {
   DevBuf files_d, blk_off, blk_size, blk_state, scan_tmp, run_start, small;  // small: err, totals, counters...
   KeyBufs dec, mrg;
   DevBuf splits, tile_state, snaps_d;
-  DevBuf esz, eshared, tstat, nxt, disk, rows, tstate, grows, gstate, gflag, gsync, idx_contrib, idx_contrib_off, blocks, files_rec, idx_esz, idx_eoff, idx_sep, out_buf, out_base_d;
+  DevBuf esz, eshared, tstat, nxt, disk, rows, tstate, grows, gstate, gflag, gsync, blocks, files_rec, idx_esz, idx_eoff, idx_sep, out_buf, out_base_d;
   uint64_t n_total = 0, n_out = 0, nblk_in = 0, nblocks_out = 0;
   uint32_t nfiles_out = 0, nruns = 0;
-  DevBuf bloom_contrib, bloom_contrib_off;  // scratch of the filter blocks' checksums
+  DevBuf cksum_contrib, cksum_contrib_off;  // scratch of the index and filter blocks' checksums
   DevBuf bloom_hashes;                      // key hashes of the output entries (filter policy jobs)
   DevBuf kv_arena, kv_offs, kv_klens;  // b200c_job_encode_kv: the caller's records on the device
   DevBuf run_bounds, run_first_d;  // [begin[K] | end[K]] of the sorted runs in the decoded columns; first file of each run
@@ -540,14 +540,14 @@ int write_tails(b200c_job* j, const std::vector<FileRec>& frs, const std::vector
     ti.format_version = P.format_version;
     ti.data_size = fr.data_size;
     ti.index_size = fr.index_size;
-    ti.filter_size = fr.filter_bytes ? fr.filter_bytes - 5 : 0;
+    ti.filter_size = fr.filter_len();
     ti.filter_entries = fr.filter_entries;
     ti.num_entries = fr.n_entries;
     ti.num_deletions = fr.num_deletions;
     ti.raw_key_size = fr.raw_key_size;
     ti.raw_value_size = fr.raw_value_size;
     ti.num_data_blocks = fr.n_blocks;
-    ti.index_key_is_user_key = !fr.index_has_seq && P.format_version > 2;
+    ti.index_key_is_user_key = fr.index_key_is_user_key(P.format_version);
     ti.column_family_id = P.column_family_id;
     ti.column_family_name = j->cf_name;
     ti.db_id = j->db_id;
@@ -558,7 +558,7 @@ int write_tails(b200c_job* j, const std::vector<FileRec>& frs, const std::vector
     ti.file_creation_time = j->fct.empty() ? 0 : j->fct[std::min<size_t>(f, j->fct.size() - 1)];
     ti.orig_file_number = P.first_file_number + f;
     std::vector<uint8_t> tail = build_output_tail(ti);
-    const uint64_t tail_off = fr.data_size + fr.filter_bytes + fr.index_size + 5;
+    const uint64_t tail_off = fr.tail_start();
     if (tail_off + tail.size() > base_off[f + 1] - base_off[f]) return fail(B200C_ERR_CUDA, "internal: output image overflow");
     const size_t so = (size_t)f * 4096;
     if (tail.size() > 4096) return fail(B200C_ERR_CUDA, "internal: tail larger than its staging slot");
@@ -609,13 +609,13 @@ int paranoid_reread(b200c_job* j, KeyCols mcols, const std::vector<FileRec>& frs
     memset(&d, 0, sizeof d);
     d.base = j->out_buf.as<uint8_t>() + base_off[f];
     d.len = j->outputs[f].meta.file_size;
-    d.index_off = fr.data_size + fr.filter_bytes;
+    d.index_off = fr.index_start();
     d.index_size = (uint32_t)fr.index_size;
     d.value_delta = P.format_version >= 4;
     d.cksum = P.checksum;
     d.gblk_first = g;
     d.nblocks = (uint32_t)fr.n_blocks;
-    d.index_user_key = (!fr.index_has_seq && P.format_version > 2) ? 1u : 0u;
+    d.index_user_key = fr.index_key_is_user_key(P.format_version) ? 1u : 0u;
     g += d.nblocks;
     maxb = std::max(maxb, d.nblocks);
     ofd[f] = d;
@@ -657,6 +657,16 @@ int paranoid_reread(b200c_job* j, KeyCols mcols, const std::vector<FileRec>& frs
   return B200C_OK;
 }
 
+// First XXH3 contribution slot (8 u64 per full 1024-byte block) of every file's index block, at [f], and filter block, at
+// [nfiles + f], in one scratch; the total behind them.  The two blocks of a file are checksummed concurrently on two streams: their
+// regions do not overlap.  The index block is sized by its bound: its length is not known yet.
+static std::vector<uint64_t> file_block_contrib_offsets(const std::vector<FileRec>& frs) {
+  const size_t n = frs.size();
+  std::vector<uint64_t> off(2 * n + 1, 0);
+  for (size_t i = 0; i < 2 * n; i++) off[i + 1] = off[i] + (i < n ? frs[i].index_bound() : frs[i - n].filter_len()) / 1024 + 1;
+  return off;
+}
+
 int encode_stage(b200c_job* j, KeyCols mcols, uint64_t n_out, uint32_t min_s1, uint32_t max_s1, EncodeWork& W, uint32_t* err, uint64_t* small) {
   const b200c_params& P = j->p;
   cudaStream_t st = j->st;
@@ -689,8 +699,7 @@ int encode_stage(b200c_job* j, KeyCols mcols, uint64_t n_out, uint32_t min_s1, u
       if (int rc = upload_small(j, j->gp_size_d.p, j->gp_size.data(), 8 * (size_t)G)) return rc;
       if (int rc = upload_small(j, j->gp_same_d.p, j->gp_same.data(), G)) return rc;
       uint64_t* ranks = j->gp_ranks_d.as<uint64_t>();
-      launch_gp_ranks(mcols, keys, keys + G, G, ranks, ranks + G, ranks + 2 * G, st);
-      j->launches += 1;
+      launch_gp_ranks(mcols, keys, keys + G, G, ranks, ranks + G, ranks + 2 * G, st, &j->launches);
       ep.gp.n = G;
       ep.gp.dynamic_file_size = P.level_compaction_dynamic_file_size;
       ep.gp.lo = ranks;
@@ -711,9 +720,8 @@ int encode_stage(b200c_job* j, KeyCols mcols, uint64_t n_out, uint32_t min_s1, u
       CU(cudaMemsetAsync(pev + cap, 0, 8 * (1 + ptiles), st));
       j->kt_begin("encode.partition_events");
       launch_partition_events(mcols, plen, cap, reinterpret_cast<uint32_t*>(pev + cap), reinterpret_cast<unsigned long long*>(pev + cap + 1),
-                              pev, err, st);
+                              pev, err, st, &j->launches);
       j->kt_end();
-      j->launches += 1;
       ep.gp.pev = pev;
       ep.gp.np = cap;
     }
@@ -760,7 +768,7 @@ int encode_stage(b200c_job* j, KeyCols mcols, uint64_t n_out, uint32_t min_s1, u
       j->kt_end(slot, j->st2);
     }
     j->kt_begin("encode.tables");
-    launch_encode_tables(mcols, ep, W, etiles, hc, max_s1, st);
+    launch_encode_tables(mcols, ep, W, etiles, hc, max_s1, st, &j->launches);
     j->kt_end();
     {
       const size_t slot = j->kt_begin("~encode.stitch_retry", j->st2);
@@ -772,13 +780,12 @@ int encode_stage(b200c_job* j, KeyCols mcols, uint64_t n_out, uint32_t min_s1, u
     j->kt_begin("encode.tilestate");
     launch_encode_tilestate(mcols, W, etiles, hc, err, st, &j->launches);
     j->kt_end();
-    j->launches += 1;
     if (P.bloom_millibits_per_key) {  // filter entries per file decide where each file's index block starts
       j->kt_begin("encode.bloom_count");
       CU(j->bloom_hashes.reserve(8 * (n_out + 1)));  // XXPH3 of every output key: computed once, read by the slices of the filter build
-      launch_bloom_count(mcols, n_out, W.files, small + kSlotTotals + 1, P.bloom_millibits_per_key, j->bloom_hashes.as<uint64_t>(), j->sms, st);
+      launch_bloom_count(mcols, n_out, W.files, small + kSlotTotals + 1, P.bloom_millibits_per_key, j->bloom_hashes.as<uint64_t>(), j->sms, st,
+                         &j->launches);
       j->kt_end();
-      j->launches += 2;
     }
     if (int rc = checked_sync(j, h, W.files, &frs)) return rc;  // sync #2: number of blocks / files, per-file records
     const uint64_t nblocks = j->nblocks_out = h[kSlotTotals];
@@ -796,24 +803,21 @@ int encode_stage(b200c_job* j, KeyCols mcols, uint64_t n_out, uint32_t min_s1, u
     // synchronise the device
     CU(j->pin_tails.reserve((size_t)nfiles * 4096 + 64));
     CU(j->pin_small.reserve(sizeof(TailCopy) * nfiles));
-    // image layout: data blocks | index block (<= 45 B per data block + 9) | tail (properties, metaindex, footer)
     base_off.resize(nfiles + 1);
     uint64_t off = 0;
     for (uint32_t f = 0; f < nfiles; f++) {
       base_off[f] = off;
-      uint64_t cap = frs[f].data_size + frs[f].filter_bytes + frs[f].n_blocks * 48 + 64 + 4096;
-      off += (cap + 255) & ~255ull;
+      off += (frs[f].image_bound(4096) + 255) & ~255ull;  // the tail is at most 4096 bytes (write_tails)
     }
     base_off[nfiles] = off;
     CU(j->out_buf.reserve(off + 256));
-    {  // scratch for the parallel part of the index-block checksum
-      std::vector<uint64_t> coff(nfiles + 1, 0);
-      for (uint32_t f = 0; f < nfiles; f++) coff[f + 1] = coff[f] + (frs[f].n_blocks * 48 + 64) / 1024 + 1;
-      CU(j->idx_contrib.reserve(64 * (coff[nfiles] + 1)));
-      CU(j->idx_contrib_off.reserve(8 * (nfiles + 1)));
-      if (int rc = upload_small(j, j->idx_contrib_off.p, coff.data(), 8 * (nfiles + 1))) return rc;  // (copied into pinned staging)
-      W.idx_contrib = j->idx_contrib.as<uint64_t>();
-      W.idx_contrib_off = j->idx_contrib_off.as<uint64_t>();
+    {  // scratch for the parallel part of the index and filter blocks' checksums
+      const std::vector<uint64_t> coff = file_block_contrib_offsets(frs);
+      CU(j->cksum_contrib.reserve(64 * (coff.back() + 1)));
+      CU(j->cksum_contrib_off.reserve(8 * coff.size()));
+      if (int rc = upload_small(j, j->cksum_contrib_off.p, coff.data(), 8 * coff.size())) return rc;  // (copied into pinned staging)
+      W.cksum_contrib = j->cksum_contrib.as<uint64_t>();
+      W.cksum_contrib_off = j->cksum_contrib_off.as<uint64_t>();
     }
     std::vector<uint8_t*> bases(nfiles);
     for (uint32_t f = 0; f < nfiles; f++) bases[f] = j->out_buf.as<uint8_t>() + base_off[f];
@@ -821,23 +825,22 @@ int encode_stage(b200c_job* j, KeyCols mcols, uint64_t n_out, uint32_t min_s1, u
     if (int rc = upload_small(j, j->out_base_d.p, bases.data(), 8 * nfiles)) return rc;
     uint8_t* const* out_base_d = j->out_base_d.as<uint8_t*>();
     j->kt_begin("encode.blocklist");
-    launch_encode_blocklist(mcols, ep, W, etiles, nblocks, err, st);
+    launch_encode_blocklist(mcols, ep, W, etiles, nblocks, err, st, &j->launches);
     j->kt_end();
     // The file tails (write_tails) need only the per-file records: statistics, boundary keys, index-block sizes.  Those kernels
     // run on the main stream in front of the emit kernel (behind it they would wait for its last CTA, see
     // launch_encode_emit); the records are gathered right behind them, and the host builds the tails while the data blocks are emitted.
     j->kt_begin("encode.filestats+index_size");
     launch_encode_index_size(mcols, ep, W, nblocks, j->sms, st, &j->launches);
-    launch_encode_filestats(mcols, W, nfiles, st);
+    launch_encode_filestats(mcols, W, nfiles, st, &j->launches);
     j->kt_end();
     if (int rc = gather_small(j, W.files)) return rc;
     CU(cudaEventRecord(j->evx[2], st));
     uint64_t data_bytes = 0;
     for (uint32_t f = 0; f < nfiles; f++) data_bytes += frs[f].data_size;
     j->kt_begin("encode.emit");
-    launch_encode_emit(mcols, ep, W, nblocks, out_base_d, data_bytes, j->sms, st);
+    launch_encode_emit(mcols, ep, W, nblocks, out_base_d, data_bytes, j->sms, st, &j->launches);
     j->kt_end();
-    j->launches += 3;
     // The index blocks are written on the side stream beside the emit kernel (a file's index block lies behind its data and filter
     // blocks: disjoint bytes).  They are enqueued after the emit so that the main stream does not idle while the host enqueues them.
     CU(cudaStreamWaitEvent(j->st2, j->evx[2], 0));
@@ -849,20 +852,11 @@ int encode_stage(b200c_job* j, KeyCols mcols, uint64_t n_out, uint32_t min_s1, u
     CU(cudaEventRecord(j->evx[3], j->st2));
     if (P.bloom_millibits_per_key) {
       j->kt_begin("encode.bloom_build");
-      // scratch for the parallel part of the filter blocks' checksums: 8 u64 per full 1024-byte block
-      std::vector<uint64_t> boff(nfiles + 1, 0);
       uint64_t max_fb = 0;
-      for (uint32_t f = 0; f < nfiles; f++) {
-        boff[f + 1] = boff[f] + frs[f].filter_bytes / 1024 + 1;
-        max_fb = std::max<uint64_t>(max_fb, frs[f].filter_bytes);
-      }
-      CU(j->bloom_contrib.reserve(64 * (boff[nfiles] + 1)));
-      CU(j->bloom_contrib_off.reserve(8 * (nfiles + 1)));
-      if (int rc = upload_small(j, j->bloom_contrib_off.p, boff.data(), 8 * (nfiles + 1))) return rc;
-      launch_bloom_build(j->bloom_hashes.as<uint64_t>(), n_out, W.files, nfiles, (uint32_t)std::min<uint64_t>(max_fb, 0xffffffffull), P.bloom_millibits_per_key, P.checksum,
-                         out_base_d, j->bloom_contrib.as<uint64_t>(), j->bloom_contrib_off.as<uint64_t>(), st);
+      for (uint32_t f = 0; f < nfiles; f++) max_fb = std::max<uint64_t>(max_fb, frs[f].filter_bytes);
+      launch_bloom_build(j->bloom_hashes.as<uint64_t>(), n_out, W, nfiles, (uint32_t)std::min<uint64_t>(max_fb, 0xffffffffull), P.bloom_millibits_per_key,
+                         P.checksum, out_base_d, st, &j->launches);
       j->kt_end();
-      j->launches += 3;
     }
     // sync #3 waits for the records gathered in front of the emit kernel only.  The error word the emit, index and filter kernels
     // may still raise is checked by finish_run().

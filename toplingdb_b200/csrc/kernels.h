@@ -155,18 +155,19 @@ struct EncodeParams {
 using GpKey = BoundKey;       // grandparent boundary key in column form
 // ---- full Bloom filter block (bloom_rules.h).  count: per file the number of entries whose key hash differs from the predecessor's
 // (XXPH3FilterBitsBuilder::AddKey drops consecutive duplicates) and from it the block size; build: set the bits, metadata, trailer.
-void launch_bloom_count(KeyCols m, uint64_t n, FileRec* files, const uint64_t* nfiles_dev, uint32_t millibits, uint64_t* hashes, int sms, cudaStream_t st);
-// max_filter_bytes: largest filter_bytes of a file (grid sizing); contrib / contrib_off: scratch for the parallel part of the XXH3 of
-// every filter block (8 u64 per full 1024-byte block; per file its first slot)
-void launch_bloom_build(const uint64_t* hashes, uint64_t n, const FileRec* files, uint32_t nfiles, uint32_t max_filter_bytes, uint32_t millibits, uint32_t cksum,
-                        uint8_t* const* out_base, uint64_t* contrib, const uint64_t* contrib_off, cudaStream_t st);
+void launch_bloom_count(KeyCols m, uint64_t n, FileRec* files, const uint64_t* nfiles_dev, uint32_t millibits, uint64_t* hashes, int sms, cudaStream_t st,
+                        uint64_t* launches);
+// max_filter_bytes: largest filter_bytes of a file (grid sizing); the checksums use w.files and w.cksum_contrib*
+struct EncodeWork;
+void launch_bloom_build(const uint64_t* hashes, uint64_t n, const EncodeWork& w, uint32_t nfiles, uint32_t max_filter_bytes, uint32_t millibits,
+                        uint32_t cksum, uint8_t* const* out_base, cudaStream_t st, uint64_t* launches);
 // fixed-prefix partitioner: the merged entries in front of which it cuts (gp_rules.h), ascending, into ev[0, cap); ev must hold ~0
 // and ticket / state (partition_event_tiles(m.n) words) zero beforehand.  More than cap events set kErrTooManyFiles.
 uint64_t partition_event_tiles(uint64_t n);
 void launch_partition_events(KeyCols m, uint32_t len, uint32_t cap, uint32_t* ticket, unsigned long long* state, uint64_t* ev, uint32_t* err,
-                             cudaStream_t st);
+                             cudaStream_t st, uint64_t* launches);
 void launch_gp_ranks(KeyCols m, const GpKey* smallest, const GpKey* largest, uint32_t n, uint64_t* lo, uint64_t* eq, uint64_t* hi,
-                     cudaStream_t st);
+                     cudaStream_t st, uint64_t* launches);
 struct BlockRec {            // one output data block
   uint64_t first_entry;
   uint64_t file_off;         // offset of the block payload inside its file
@@ -177,6 +178,9 @@ struct KeyRec {
   uint64_t hi, lo, tr;
   uint32_t ulen, pad;
 };
+constexpr uint32_t kBlockTrailerLen = 5;  // compression type + checksum behind every block
+// An output image is  data blocks | filter block | index block | tail (properties, metaindex, footer);  the filter and the index
+// block each carry a trailer.  The accessors below are the one statement of that layout.
 struct FileRec {             // one output file (device-computed part)
   uint64_t first_entry, n_entries;
   uint64_t first_block, n_blocks;
@@ -187,7 +191,19 @@ struct FileRec {             // one output file (device-computed part)
   KeyRec smallest, largest;
   uint32_t index_has_seq;    // some adjacent blocks share a user key => index keys keep the 8-byte trailer
   uint64_t filter_entries;   // hashes in the Bloom filter (rocksdb.num.filter_entries); 0 without a filter policy
-  uint64_t filter_bytes;     // filter block on disk: bits + 5 metadata bytes + 5 trailer bytes; sits between data and index blocks
+  uint64_t filter_bytes;     // filter block on disk: bits + 5 metadata bytes + trailer; 0 without a filter
+
+  __host__ __device__ uint64_t filter_start() const { return data_size; }
+  // filter bits + metadata, without the trailer (0: no filter block)
+  __host__ __device__ uint64_t filter_len() const { return filter_bytes ? filter_bytes - kBlockTrailerLen : 0; }
+  __host__ __device__ uint64_t index_start() const { return data_size + filter_bytes; }
+  __host__ __device__ uint64_t tail_start() const { return index_start() + index_size + kBlockTrailerLen; }
+  // the index block with its trailer takes at most this (<= 45 B per data block + 9), before index_size is known
+  __host__ __device__ uint64_t index_bound() const { return n_blocks * 48 + 64; }
+  // bytes the image needs at most with a tail of tail_bytes
+  __host__ __device__ uint64_t image_bound(uint64_t tail_bytes) const { return index_start() + index_bound() + tail_bytes; }
+  // rocksdb.index.key.is.user.key (index_builder.h:175-180): no two adjacent blocks share a user key, from format_version 3 on
+  __host__ __device__ bool index_key_is_user_key(uint32_t format_version) const { return !index_has_seq && format_version > 2; }
 };
 struct TileRow {             // block-cut transfer function of one tile for one entry-point candidate
   uint32_t exit;             // chain exit, entries past the tile end
@@ -224,31 +240,34 @@ struct EncodeWork {                  // device scratch owned by the job
   uint64_t* totals;     // [0] = number of blocks, [1] = number of files
   BlockRec* blocks;     // capacity nblk_cap
   FileRec* files;       // kMaxOutFiles
-  uint32_t* idx_esz;    // per block: encoded index entry size
-  uint64_t* idx_eoff;   // per block: exclusive scan of idx_esz (global; file-relative after subtracting the file's first)
+  uint32_t* idx_esz;    // per block: encoded index entry size without the key's 8-byte trailer (index_has_seq adds it)
+  uint64_t* idx_eoff;   // nblocks + 1: exclusive scan of idx_esz, the total behind it
   KeyRec* idx_sep;      // per block: separator key (ulen excludes the trailer; pad=1 when the trailer was replaced)
   uint64_t* scan_tmp;
-  uint64_t* idx_contrib;      // XXH3 accumulator contributions of the 1024-byte blocks of every index block (8 u64 each)
-  uint64_t* idx_contrib_off;  // per file: first contribution slot
+  // XXH3 accumulator contributions of the 1024-byte blocks of every index and filter block (8 u64 each); first slot per file:
+  // cksum_contrib_off[f] for its index block, cksum_contrib_off[nfiles + f] for its filter block (file_block_contrib_offsets)
+  uint64_t* cksum_contrib;
+  uint64_t* cksum_contrib_off;
   uint16_t* nxt;        // n: tile-relative end of the block that would start at entry i
   uint32_t* disk;       // n: on-disk bytes of that block
 };
 // TableBuilder-only path (no merge in front): sizes + statistics per kEncTile entries + their prefix array (tprefix_out)
 void launch_encode_sizes(KeyCols m, const unsigned long long* n_dev, EncodeWork w, unsigned long long* tprefix_out, uint64_t n_cap, int sms, cudaStream_t st);
-void launch_encode_tables(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t ntiles, uint32_t hc, uint32_t max_s1, cudaStream_t st);
+void launch_encode_tables(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t ntiles, uint32_t hc, uint32_t max_s1, cudaStream_t st,
+                          uint64_t* launches);
 // stitch: launched on its own stream BEFORE / alongside launch_encode_tables (it consumes groups as their gready flag appears);
 // tilestate: after both have finished
 void launch_encode_stitch(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t ntiles, uint32_t hc, uint32_t* err, uint32_t attempt,
                           uint32_t* sflag, cudaStream_t st, uint64_t* launches);
 void launch_encode_tilestate(KeyCols m, EncodeWork w, uint64_t ntiles, uint32_t hc, uint32_t* err, cudaStream_t st, uint64_t* launches);
 void launch_encode_blocklist(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t ntiles, uint64_t nblk_cap, uint32_t* err,
-                             cudaStream_t st);
+                             cudaStream_t st, uint64_t* launches);
 // per-file statistics, boundary keys and index-block size: after launch_encode_index_size
-void launch_encode_filestats(KeyCols m, EncodeWork w, uint32_t nfiles, cudaStream_t st);
+void launch_encode_filestats(KeyCols m, EncodeWork w, uint32_t nfiles, cudaStream_t st, uint64_t* launches);
 uint32_t encode_emit_slice(uint32_t block_size);
 // out_base[f] = device address where file f's image starts; data_bytes = all data blocks incl. trailers (with m.n: selects the kernel)
 void launch_encode_emit(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nblocks, uint8_t* const* out_base, uint64_t data_bytes,
-                        int sms, cudaStream_t st);
+                        int sms, cudaStream_t st, uint64_t* launches);
 // index blocks in two steps: separators, entry sizes and their scan (what the file sizes need), then the entries, restart arrays and
 // trailers written into the images
 void launch_encode_index_size(KeyCols m, EncodeParams ep, EncodeWork w, uint64_t nblocks, int sms, cudaStream_t st, uint64_t* launches);
