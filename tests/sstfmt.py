@@ -73,7 +73,9 @@ def read_block(data, handle):
     if ctype == 2:
         import zlib
         usize, p = varint(payload, 0)
-        payload = zlib.decompress(payload[p:], -14)
+        # (one inflate call over the whole announced size, as the reference's Zlib_Uncompress makes: a stream written with
+        #  window_bits -15 then reads back under -14 -- in smaller steps its matches past 16 KiB fall outside the window)
+        payload = zlib.decompress(payload[p:], -14, max(usize, 1))
         assert len(payload) == usize
     else:
         assert ctype == 0, f"block compression type {ctype}"
