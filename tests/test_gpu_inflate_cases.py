@@ -152,3 +152,11 @@ def test_reference_db_compacts_through_the_b200_executor():
         [e for f in want["outputs"] for e in sstfmt.parse_sst(f)["entries"]]
     for k in H.STAT_KEYS:
         assert gm["stats"][k] == wm["stats"][k], k
+
+
+def test_verification_adds_exactly_the_verify_launch():
+    """stats.kernel_launches of a zlib job: verify_input_checksums adds the one launch of the verify kernel and nothing else"""
+    from gpu_harness import run_product
+    c = _case("level6_default")
+    launches = {v: run_product(c["params"], c["ref"]["inputs"], verify_input_checksums=v)[2].kernel_launches for v in (1, 0)}
+    assert launches[1] == launches[0] + 1, launches

@@ -1,7 +1,8 @@
-"""toplingdb_b200/csrc/inflate_rules.h (the per-thread raw DEFLATE decoder of the device's block decompression) compiled for the host
-and checked against zlib: streams of all three block types (stored, fixed, dynamic Huffman) as the reference's Zlib_Compress writes them
-(util/compression.h:746-826: raw deflate, window_bits -14), long matches, the 16 KiB window limit, and malformed input (truncated
-streams, random bytes, output larger than the announced size) which must be refused, never overrun."""
+"""toplingdb_b200/csrc/inflate_rules.h (the raw DEFLATE decoder of the device's block decompression and of the host's compressed index
+blocks) compiled for the host and checked against zlib: streams of all three block types (stored, fixed, dynamic Huffman) as the
+reference's Zlib_Compress writes them (util/compression.h:746-826: raw deflate, window_bits -14), long matches, the 16 KiB window limit,
+and malformed input (truncated streams, random bytes, output larger than the announced size) which must be refused, never overrun.
+Also the varint32 size prefix in front of the stream, which both sides read with inf_size_prefix."""
 import ctypes as C
 import os
 import random
@@ -23,6 +24,8 @@ def sim(tmp_path_factory):
     L = C.CDLL(so)
     L.inflate_sim.restype = C.c_long
     L.inflate_sim.argtypes = [C.c_char_p, C.c_uint32, C.c_char_p, C.c_uint32]
+    L.size_prefix_sim.restype = C.c_int
+    L.size_prefix_sim.argtypes = [C.c_char_p, C.c_uint32, C.POINTER(C.c_uint64)]
     return L
 
 
@@ -96,3 +99,29 @@ def test_agrees_with_zlib_on_random_streams(sim):
         comp = _deflate(data, rnd.choice([0, 1, 6, 9]), rnd.choice([zlib.Z_DEFAULT_STRATEGY, zlib.Z_FIXED, zlib.Z_FILTERED]))
         got_n, got, _ = _inflate(sim, comp, len(data))
         assert got_n == len(data) and got == zlib.decompress(comp, -14)
+
+
+def _varint(u):
+    out = bytearray()
+    while u >= 128:
+        out.append(u & 127 | 128)
+        u >>= 7
+    return bytes(out + bytes([u]))
+
+
+def _prefix(sim, data, size=None):
+    u = C.c_uint64(0xdead)
+    n = sim.size_prefix_sim(data, len(data) if size is None else size, C.byref(u))
+    return n, u.value if n else None
+
+
+def test_size_prefix_reads_one_to_five_bytes_within_the_block(sim):
+    for u in (0, 1, 4, 8, 127, 128, 6144, 16383, 16384, (1 << 21) - 1, 1 << 21, (1 << 28) - 1, 1 << 28, 0x7fffffff, 1 << 31,
+              (1 << 32) - 1, (1 << 35) - 1):
+        enc = _varint(u)
+        assert _prefix(sim, enc + b"\x01\x02") == (len(enc), u), u  # (the stream behind the prefix is not read)
+        assert _prefix(sim, enc + b"\x01", len(enc) - 1) == (0, None), u  # cut by the block's end
+    for enc in (b"\x80" * 5 + b"\x01", b"\xff" * 6, b"\x80\x80\x80\x80\x80"):  # no end within the first five bytes
+        assert _prefix(sim, enc) == (0, None), enc
+    assert _prefix(sim, b"", 0) == (0, None)
+    assert _prefix(sim, b"\x85\x80\x80\x80\x00") == (5, 5)  # zero-padded: five bytes, as the reference's GetVarint32 reads them

@@ -205,19 +205,26 @@ struct KeyBufs {
   KeyCols cols(uint64_t n) const { return {pfx.as<ulonglong2>(), tr.as<uint64_t>(), vref.as<uint64_t>(), meta.as<uint32_t>(), n}; }
 };
 
+struct HostCopy {  // the device copy of a host input (stage_input)
+  DevBuf buf;
+  cudaEvent_t done = nullptr;  // recorded behind the last copy into buf, on the stream that made it (nullptr: no copy yet)
+  bool fresh = false;          // b200c_job_add_input's eager copy: the next run consumes it (later runs copy anew: the host buffer may change)
+};
+struct IndexBlock {            // the index block of an input as the host reads it (input_index_block)
+  const uint8_t* p = nullptr;  // into a host image, or into buf: the block read from device memory, or inflated
+  uint64_t len = 0;
+  bool inflated = false;
+  std::vector<uint8_t> buf;
+};
 struct Input {
   int level;
   uint64_t file_number;
   const uint8_t* data;
   uint64_t len;
   int mem_kind;
-  DevBuf staged;  // device copy of a host input
-  cudaEvent_t up_ev = nullptr;  // eager upload (started by b200c_job_add_input on the copy stream) has finished
-  bool uploaded = false;        // the staged copy is current for the NEXT run (consumed by it)
-  bool shared_copy = false;     // the staged copy is complete and in use by sub-jobs (b200c_job_create_sub)
-  DevBuf index_inflated;        // device copy of an index block that was stored compressed
-  std::vector<uint8_t> index_host;  // ... and its host bytes (source of the upload; kept until the run ends)
-  const uint8_t* dev = nullptr;
+  HostCopy copy;
+  IndexBlock index;       // a compressed input's index block, read by run_job (the source of the upload; kept until the run ends)
+  DevBuf index_inflated;  // ... its device copy when it was inflated
   InputTail tail;
 };
 constexpr uint64_t kTailFetch = 4096;  // bytes read from the end of an input: footer + metaindex + properties live there
@@ -341,39 +348,37 @@ bool trailer_ok(const Input& in, const uint8_t* blk, uint64_t size, const uint8_
   return !in.tail.checksum_type || host_block_checksum(in.tail.checksum_type, blk, size, trailer[0]) == stored;
 }
 
-int fetch_tail(b200c_job* j, Input& in, const uint8_t* prefetched = nullptr) {
-  // footer, metaindex, properties: three tiny reads (D2H when the image lives in device memory)
-  auto read = [&](uint64_t off, uint64_t n, std::vector<uint8_t>& buf) -> int {
-    buf.resize(n);
-    if (in.mem_kind == B200C_MEM_HOST) {
-      memcpy(buf.data(), in.data + off, n);
-    } else {
-      CU(cudaMemcpyAsync(buf.data(), in.data + off, n, cudaMemcpyDeviceToHost, j->st));
-      CU(cudaStreamSynchronize(j->st));
-    }
+// Bytes [off, off + n) of an input image for the host: *p points into a host image, or into *buf, where they are copied from a
+// device image on the job's stream (behind its wait_ev: job_bind).
+int read_image(b200c_job* j, const Input& in, uint64_t off, uint64_t n, std::vector<uint8_t>* buf, const uint8_t** p) {
+  *p = in.data + off;
+  if (in.mem_kind == B200C_MEM_HOST) return B200C_OK;
+  buf->resize(n);
+  CU(cudaMemcpyAsync(buf->data(), *p, n, cudaMemcpyDeviceToHost, j->st));
+  CU(cudaStreamSynchronize(j->st));
+  *p = buf->data();
+  return B200C_OK;
+}
+
+// The tail of an input -- footer, metaindex, properties -- into in.tail, and every refusal of a single input.  tp: the last
+// kTailFetch bytes of a device image, already read (run_job reads those of all its device images in one batch).
+int open_input(b200c_job* j, Input& in, const uint8_t* tp = nullptr) {
+  if (in.len < 53) return fail(B200C_ERR_CORRUPTION, "input shorter than a footer");
+  const uint64_t tail_off = in.len - std::min<uint64_t>(in.len, kTailFetch);
+  std::vector<uint8_t> tail, tmp;
+  if (!tp)
+    if (int rc = read_image(j, in, tail_off, in.len - tail_off, &tail, &tp)) return rc;
+  // bytes [off, off + n) of the image, n <= len - off: inside its tail, or read on their own
+  auto view = [&](uint64_t off, uint64_t n, const uint8_t** p) -> int {
+    if (off < tail_off) return read_image(j, in, off, n, &tmp, p);
+    *p = tp + (off - tail_off);
     return B200C_OK;
   };
-  if (in.len < 53) return fail(B200C_ERR_CORRUPTION, "input shorter than a footer");
-  const uint64_t tail_n = std::min<uint64_t>(in.len, kTailFetch);
-  std::vector<uint8_t> tail, tmp;
-  int rc = B200C_OK;
-  if (prefetched) tail.assign(prefetched, prefetched + tail_n);  // device image: fetched together with the other inputs' tails
-  else rc = read(in.len - tail_n, tail_n, tail);
-  if (rc) return rc;
-  std::string e = parse_footer(tail.data() + tail_n - 53, in.len, &in.tail);
-  if (!e.empty()) return fail(B200C_ERR_CORRUPTION, e);
-  auto view = [&](uint64_t off, uint64_t n, const uint8_t** p) -> int {
-    if (off >= in.len - tail_n && off + n <= in.len) {
-      *p = tail.data() + (off - (in.len - tail_n));
-      return B200C_OK;
-    }
-    int r = read(off, n, tmp);
-    *p = tmp.data();
-    return r;
-  };
   const uint8_t* blk;
-  rc = view(in.tail.meta_off, in.tail.meta_size + 5, &blk);
-  if (rc) return rc;
+  if (int rc = view(in.len - 53, 53, &blk)) return rc;
+  std::string e = parse_footer(blk, in.len, &in.tail);
+  if (!e.empty()) return fail(B200C_ERR_CORRUPTION, e);
+  if (int rc = view(in.tail.meta_off, in.tail.meta_size + 5, &blk)) return rc;
   if (!trailer_ok(in, blk, in.tail.meta_size, blk + in.tail.meta_size)) return fail(B200C_ERR_CORRUPTION, "metaindex block checksum mismatch");
   std::map<std::string, std::pair<uint64_t, uint64_t>> meta;
   e = parse_metaindex(blk, in.tail.meta_size, &meta);
@@ -388,8 +393,7 @@ int fetch_tail(b200c_job* j, Input& in, const uint8_t* prefetched = nullptr) {
   in.tail.props_off = it->second.first;
   in.tail.props_size = it->second.second;
   if (in.tail.props_off + in.tail.props_size + 5 > in.len) return fail(B200C_ERR_CORRUPTION, "properties handle out of range");
-  rc = view(in.tail.props_off, in.tail.props_size + 5, &blk);
-  if (rc) return rc;
+  if (int rc = view(in.tail.props_off, in.tail.props_size + 5, &blk)) return rc;
   // num_entries / num_data_blocks from this block size every device buffer: its checksum is verified like the metaindex block's
   if (!trailer_ok(in, blk, in.tail.props_size, blk + in.tail.props_size)) return fail(B200C_ERR_CORRUPTION, "properties block checksum mismatch");
   e = parse_properties(blk, in.tail.props_size, &in.tail);
@@ -405,65 +409,54 @@ int fetch_tail(b200c_job* j, Input& in, const uint8_t* prefetched = nullptr) {
   if (!in.tail.comparator_name.empty() && in.tail.comparator_name != "leveldb.BytewiseComparator")
     return fail(B200C_ERR_NOT_SUPPORTED, "comparator " + in.tail.comparator_name + " (only leveldb.BytewiseComparator runs on the device)");
   if (in.tail.num_data_blocks > 0xffffffffull) return fail(B200C_ERR_NOT_SUPPORTED, "too many data blocks");
+  if (in.mem_kind != B200C_MEM_HOST && ((uintptr_t)in.data & 15)) return fail(B200C_ERR_INVALID_ARGUMENT, "device input images must be 16-byte aligned");
+  if (in.tail.index_size > 0xffffffffull) return fail(B200C_ERR_NOT_SUPPORTED, "index block >= 4 GiB");
   return B200C_OK;
 }
 
 bool input_is_compressed(const Input& in) { return !in.tail.compression_name.empty() && in.tail.compression_name != "NoCompression"; }
-// The index block of a file written with block compression goes through the same WriteBlock as data blocks (enable_index_compression,
-// block_based_table_builder.cc:1566-1573).  It is O(blocks) metadata that the host reads anyway (tail, ranges): a compressed one is
-// inflated here, with the product's own decoder (inflate_rules.h compiled for the host), after its checksum is verified.
-// *out is left empty when the block is stored uncompressed.
-int host_inflated_index(const Input& in, std::vector<uint8_t>* out) {
-  out->clear();
-  const uint64_t off = in.tail.index_off, size = in.tail.index_size;
-  if (off + size + 5 > in.len) return fail(B200C_ERR_CORRUPTION, "index handle out of range");
-  uint8_t trailer[5];
-  if (in.mem_kind == B200C_MEM_HOST) memcpy(trailer, in.data + off + size, 5);
-  else CU(cudaMemcpy(trailer, in.data + off + size, 5, cudaMemcpyDeviceToHost));
-  if (trailer[0] == 0) return B200C_OK;
-  if (trailer[0] != 2) return fail(B200C_ERR_NOT_SUPPORTED, "index block compressed with a codec the device path does not decode");
-  std::vector<uint8_t> comp;
-  const uint8_t* cp = in.data + off;
-  if (in.mem_kind != B200C_MEM_HOST) {
-    comp.resize(size);
-    CU(cudaMemcpy(comp.data(), in.data + off, size, cudaMemcpyDeviceToHost));
-    cp = comp.data();
-  }
-  if (!trailer_ok(in, cp, size, trailer)) return fail(B200C_ERR_CORRUPTION, "index block checksum mismatch");
+// The index block of an opened input.  A file written with block compression stores it through the same WriteBlock as its data
+// blocks (enable_index_compression, block_based_table_builder.cc:1566-1573): O(blocks) metadata that the host reads anyway, so a
+// compressed one is inflated here (inflate_rules.h compiled for the host) once its checksum is verified.  It may announce
+// 8 <= u <= 2^31 bytes: 8 is the smallest index block (a restart offset and the restart count; the device's index decoder refuses
+// less).  A data block has its own bounds (decode.cu compressed_prefix); the upper bounds' difference of one is kept as it was.
+int input_index_block(b200c_job* j, const Input& in, IndexBlock* out) {
+  const uint64_t size = in.tail.index_size;
+  out->len = size;
+  out->inflated = false;
+  if (int rc = read_image(j, in, in.tail.index_off, size + 5, &out->buf, &out->p)) return rc;  // (inside the image: parse_footer)
+  const uint8_t* trailer = out->p + size;
+  if (!input_is_compressed(in) || trailer[0] == 0) return B200C_OK;
+  if (trailer[0] != kZlibCompressionType)
+    return fail(B200C_ERR_NOT_SUPPORTED, "index block compressed with a codec the device path does not decode");
+  if (!trailer_ok(in, out->p, size, trailer)) return fail(B200C_ERR_CORRUPTION, "index block checksum mismatch");
   uint64_t u = 0;
-  uint32_t h = 0;
-  for (int sft = 0; h < 5 && h < size; sft += 7) {
-    const uint8_t c = cp[h++];
-    u |= (uint64_t)(c & 127) << sft;
-    if (c < 128) break;
-  }
-  if (u < 8 || u > (1ull << 31)) return fail(B200C_ERR_CORRUPTION, "compressed index block announces a bad size");
-  out->resize(u);
+  const int h = inf_size_prefix(out->p, (uint32_t)size, &u);
+  if (h == 0 || u < 8 || u > (1ull << 31)) return fail(B200C_ERR_CORRUPTION, "compressed index block announces a bad size");
+  std::vector<uint8_t> raw((size_t)u);
   std::unique_ptr<b200c::InfWork> iw(new b200c::InfWork);
-  if (b200c::inflate_raw(cp + h, (uint32_t)(size - h), out->data(), (uint32_t)u, iw.get()) != (long)u)
+  if (b200c::inflate_raw(out->p + h, (uint32_t)(size - h), raw.data(), (uint32_t)u, iw.get()) != (long)u)
     return fail(B200C_ERR_CORRUPTION, "compressed index block does not inflate to its announced size");
+  out->buf.swap(raw);
+  out->p = out->buf.data();
+  out->len = u;
+  out->inflated = true;
   return B200C_OK;
 }
 
-// The index block of an input, readable on the host: *blk points into the image, or into *buf when the block was inflated or
-// copied from device memory.
-int host_index_block(const Input& in, std::vector<uint8_t>* buf, const uint8_t** blk, uint64_t* len) {
-  if (in.tail.index_off + in.tail.index_size + 5 > in.len) return fail(B200C_ERR_CORRUPTION, "index handle out of range");
-  buf->clear();
-  if (input_is_compressed(in))
-    if (int rc = host_inflated_index(in, buf)) return rc;
-  if (!buf->empty()) {
-    *blk = buf->data();
-    *len = buf->size();
+// Hands stream s the device copy of host input `in`.  With reuse and a copy made before (by any writer), s waits for it; otherwise
+// bytes [lo, hi) are copied on s, and `done` is recorded behind them.
+int stage_input(Input& in, cudaStream_t s, bool reuse, uint64_t lo = 0, uint64_t hi = ~0ull) {
+  HostCopy& c = in.copy;
+  if (reuse && c.done) {
+    CU(cudaStreamWaitEvent(s, c.done, 0));
     return B200C_OK;
   }
-  *blk = in.data + in.tail.index_off;
-  *len = in.tail.index_size;
-  if (in.mem_kind != B200C_MEM_HOST) {
-    buf->resize(*len);
-    CU(cudaMemcpy(buf->data(), *blk, *len, cudaMemcpyDeviceToHost));
-    *blk = buf->data();
-  }
+  hi = std::min(hi, in.len);
+  CU(c.buf.reserve(in.len + 64));
+  if (hi > lo) CU(cudaMemcpyAsync(c.buf.p + lo, in.data + lo, hi - lo, cudaMemcpyHostToDevice, s));
+  if (!c.done) CU(cudaEventCreateWithFlags(&c.done, cudaEventDisableTiming));
+  CU(cudaEventRecord(c.done, s));
   return B200C_OK;
 }
 
@@ -639,13 +632,13 @@ int paranoid_reread(b200c_job* j, KeyCols mcols, const std::vector<FileRec>& frs
   CU(cudaMemsetAsync(j->blk_state.p, 0, 8 * (nblocks + 1), st));
   const FileDesc* vf = j->vfiles_d.as<FileDesc>();
   j->kt_begin("verify.reread");
-  launch_index_decode(vf, (int)nfiles, maxb, j->blk_off.as<uint64_t>(), j->blk_size.as<uint32_t>(), BoundKey{}, 0, BoundKey{}, 0, err, st);
+  launch_index_decode(vf, (int)nfiles, maxb, j->blk_off.as<uint64_t>(), j->blk_size.as<uint32_t>(), BoundKey{}, 0, BoundKey{}, 0, err, st,
+                      &j->launches);
   launch_block_decode_fused(vf, (int)nfiles, j->blk_off.as<uint64_t>(), j->blk_size.as<uint32_t>(), (uint32_t)nblocks, 1, n_out, j->dec.mut(),
                             j->blk_state.as<unsigned long long>(), reinterpret_cast<uint32_t*>(small + kSlotDecTicket),
-                            j->vrun_start.as<uint64_t>(), small + kSlotTotalIn, err, j->sms, st);
-  launch_compare_columns(mcols, j->dec.cols(n_out), n_out, err, j->sms, st);
+                            j->vrun_start.as<uint64_t>(), small + kSlotTotalIn, err, j->sms, st, &j->launches);
+  launch_compare_columns(mcols, j->dec.cols(n_out), n_out, err, j->sms, st, &j->launches);
   j->kt_end();
-  j->launches += 3;
   uint64_t hv[kSmallSlots];
   if (int rc = read_small(j, hv)) return rc;
   if ((uint32_t)hv[kSlotErr] & ~(uint32_t)kFlagHasSingleDelete) {  // whatever the reader tripped over, the file is not what was written
@@ -924,21 +917,25 @@ int encode_columns(b200c_job* j, uint64_t n, const void* pfx, const void* tr, co
 int run_merge_encode(b200c_job* j, int until, KeyCols decc, RunBounds runs, uint64_t n_decoded, uint64_t N, bool clipped,
                      uint64_t range_value_bytes, uint64_t* small, uint32_t* err);
 
-int job_prepare(b200c_job* j) {
+// The job's device, streams and events (made on first use).  A sub-job of a range-pipelined parent: st waits for the uploads of its
+// part of the inputs before anything reads them.
+int job_bind(b200c_job* j) {
   CU(cudaSetDevice(j->p.device));
   if (!j->st) {
     CU(cudaStreamCreateWithFlags(&j->st, cudaStreamNonBlocking));
-    {
-      int prio_lo = 0, prio_hi = 0;
-      CU(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
-      CU(cudaStreamCreateWithPriority(&j->st2, cudaStreamNonBlocking, prio_hi));
-    }
+    int prio_lo = 0, prio_hi = 0;
+    CU(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
+    CU(cudaStreamCreateWithPriority(&j->st2, cudaStreamNonBlocking, prio_hi));
     for (auto& e : j->ev) CU(cudaEventCreate(&e));
     for (auto& e : j->evx) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
-    cudaDeviceProp prop;
-    CU(cudaGetDeviceProperties(&prop, j->p.device));
-    j->sms = prop.multiProcessorCount;
+    CU(cudaDeviceGetAttribute(&j->sms, cudaDevAttrMultiProcessorCount, j->p.device));
   }
+  if (j->wait_ev) CU(cudaStreamWaitEvent(j->st, j->wait_ev, 0));
+  return B200C_OK;
+}
+
+int job_prepare(b200c_job* j) {
+  if (int rc = job_bind(j)) return rc;
   j->outputs.clear();
   j->stage_done = 0;
   j->launches = 0;
@@ -954,7 +951,6 @@ int run_job(b200c_job* j, int until) {
   const b200c_params& P = j->p;
   if (int rc = job_prepare(j)) return rc;
   cudaStream_t st = j->st;
-  if (j->wait_ev) CU(cudaStreamWaitEvent(st, j->wait_ev, 0));  // sub-job of a range-pipelined parent: its part of the inputs is on its way
   const int k = (int)j->inputs.size();
   if (k == 0) return fail(B200C_ERR_INVALID_ARGUMENT, "job has no inputs");
 
@@ -979,23 +975,14 @@ int run_job(b200c_job* j, int until) {
   }
   for (int i = 0; i < k; i++) {
     Input& in = j->inputs[i];
-    int rc = fetch_tail(j, in, in.mem_kind != B200C_MEM_HOST && in.len >= 53 ? j->pin_small.p + (size_t)i * kTailFetch : nullptr);
-    if (rc) return rc;
-    if (in.mem_kind == B200C_MEM_HOST) {
-      if (in.uploaded) {  // b200c_job_add_input already started the copy (it overlapped the caller's file reads)
-        CU(cudaStreamWaitEvent(st, in.up_ev, 0));
-        in.uploaded = false;  // a later run of the same job copies again: the host buffer may have changed
-      } else {
-        CU(in.staged.reserve(in.len + 64));
-        CU(cudaMemcpyAsync(in.staged.p, in.data, in.len, cudaMemcpyHostToDevice, st));
-      }
-      in.dev = in.staged.as<uint8_t>();
-    } else {
-      if ((uintptr_t)in.data & 15) return fail(B200C_ERR_INVALID_ARGUMENT, "device input images must be 16-byte aligned");
-      in.dev = in.data;
+    const bool host = in.mem_kind == B200C_MEM_HOST;
+    if (int rc = open_input(j, in, host ? nullptr : j->pin_small.p + (size_t)i * kTailFetch)) return rc;
+    if (host) {  // b200c_job_add_input's eager copy once (it overlapped the caller's file reads), else a new one
+      if (int rc = stage_input(in, st, in.copy.fresh)) return rc;
+      in.copy.fresh = false;
     }
     FileDesc& fd = fds[i];
-    fd.base = in.dev;
+    fd.base = host ? in.copy.buf.as<uint8_t>() : in.data;
     fd.len = in.len;
     fd.index_off = in.tail.index_off;
     fd.index_size = (uint32_t)in.tail.index_size;
@@ -1003,13 +990,11 @@ int run_job(b200c_job* j, int until) {
     fd.cksum = in.tail.checksum_type;
     fd.gblk_first = (uint32_t)nblk;
     fd.nblocks = (uint32_t)in.tail.num_data_blocks;
-    fd.index_user_key = in.tail.index_key_is_user_key ? 1u : 0u;
-    fd.index_ptr = nullptr;
+    fd.index_user_key = in.tail.index_key_is_user_key ? 1u : 0u;  // (index_ptr: the vector zeroed it)
     if (input_is_compressed(in)) any_compressed = true;  // kZlibCompression: data blocks are inflated on the device, the index block below
     nblk += in.tail.num_data_blocks;
     n_props += in.tail.num_entries;
     in_bytes += in.len;
-    if (in.tail.index_size > 0xffffffffull) return fail(B200C_ERR_NOT_SUPPORTED, "index block >= 4 GiB");
   }
   if (any_compressed) {
     // compressed index blocks: inflated on the host, one thread per file (a 256 MiB file has ~3.5 MB of index: ~17 ms on one core)
@@ -1020,7 +1005,7 @@ int run_job(b200c_job* j, int until) {
       if (!input_is_compressed(j->inputs[i])) continue;
       pool.emplace_back([&, i]() {
         cudaSetDevice(P.device);
-        rcs[i] = host_inflated_index(j->inputs[i], &j->inputs[i].index_host);
+        rcs[i] = input_index_block(j, j->inputs[i], &j->inputs[i].index);
         if (rcs[i]) msgs[i] = g_err;  // (the message is per thread)
       });
     }
@@ -1028,11 +1013,11 @@ int run_job(b200c_job* j, int until) {
     for (int i = 0; i < k; i++) {
       if (rcs[i]) return fail(rcs[i], msgs[i]);
       Input& in = j->inputs[i];
-      if (!input_is_compressed(in) || in.index_host.empty()) continue;
-      CU(in.index_inflated.reserve(in.index_host.size() + 64));
-      CU(cudaMemcpyAsync(in.index_inflated.p, in.index_host.data(), in.index_host.size(), cudaMemcpyHostToDevice, st));
+      if (!input_is_compressed(in) || !in.index.inflated) continue;
+      CU(in.index_inflated.reserve(in.index.len + 64));
+      CU(cudaMemcpyAsync(in.index_inflated.p, in.index.p, in.index.len, cudaMemcpyHostToDevice, st));
       fds[i].index_ptr = in.index_inflated.as<uint8_t>();
-      fds[i].index_size = (uint32_t)in.index_host.size();
+      fds[i].index_size = (uint32_t)in.index.len;
     }
   }
   if (nblk > 0xfffffff0ull) return fail(B200C_ERR_NOT_SUPPORTED, "too many data blocks");
@@ -1068,9 +1053,8 @@ int run_job(b200c_job* j, int until) {
     j->kt_begin("decode.index");
     // a sub-compaction's key range: data blocks that cannot hold a key of [start, end) are dropped here, before anything of them is read
     launch_index_decode(files_d, k, maxb, j->blk_off.as<uint64_t>(), j->blk_size.as<uint32_t>(), j->range_lo, P.has_range_start, j->range_hi,
-                        P.has_range_end, err, st);
+                        P.has_range_end, err, st, &j->launches);
     j->kt_end();
-    j->launches++;
   }
   const uint8_t* arena = nullptr;
   if (nblk && any_compressed) {
@@ -1078,16 +1062,15 @@ int run_job(b200c_job* j, int until) {
     CU(j->cslot.reserve(4 * (nblk + 1)));
     CU(j->cslot_off.reserve(8 * (nblk + 1)));
     j->kt_begin("decode.inflate");
-    launch_block_usize(files_d, j->blk_off.as<uint64_t>(), j->blk_size.as<uint32_t>(), (uint32_t)nblk, j->cslot.as<uint32_t>(), err, st);
+    launch_block_usize(files_d, j->blk_off.as<uint64_t>(), j->blk_size.as<uint32_t>(), (uint32_t)nblk, j->cslot.as<uint32_t>(), err, st, &j->launches);
     exclusive_scan<uint32_t>(j->cslot.as<uint32_t>(), j->cslot_off.as<uint64_t>(), nblk, j->scan_tmp.as<uint64_t>(), small + kSlotArena, st, &j->launches);
     uint64_t hc[kSmallSlots];
     if (int rc = checked_sync(j, hc)) return rc;  // sync: the arena is sized by what the blocks announce
     CU(j->arena.reserve(hc[kSlotArena] + 256));
     arena = j->arena.as<uint8_t>();
     launch_inflate_blocks(files_d, j->blk_off.as<uint64_t>(), j->blk_size.as<uint32_t>(), j->cslot.as<uint32_t>(), j->cslot_off.as<uint64_t>(),
-                          (uint32_t)nblk, j->arena.as<uint8_t>(), P.verify_input_checksums, err, j->sms, st);
+                          (uint32_t)nblk, j->arena.as<uint8_t>(), P.verify_input_checksums, err, j->sms, st, &j->launches);
     j->kt_end();
-    j->launches += 3;
   }
   CU(cudaMemsetAsync(j->run_start.p, 0, 8 * (k + 1), st));  // stays zero when there is no data block at all
   if (nblk) {
@@ -1095,9 +1078,8 @@ int run_job(b200c_job* j, int until) {
     j->kt_begin("decode.blocks");
     launch_block_decode_fused(files_d, k, j->blk_off.as<uint64_t>(), j->blk_size.as<uint32_t>(), (uint32_t)nblk, P.verify_input_checksums, N,
                               j->dec.mut(), j->blk_state.as<unsigned long long>(), reinterpret_cast<uint32_t*>(small + kSlotDecTicket),
-                              j->run_start.as<uint64_t>(), small + kSlotTotalIn, err, j->sms, st, arena);
+                              j->run_start.as<uint64_t>(), small + kSlotTotalIn, err, j->sms, st, &j->launches, arena);
     j->kt_end();
-    j->launches++;
   }
   CU(cudaEventRecord(j->ev[1], st));
   const KeyCols decc = j->dec.cols(N);
@@ -1125,8 +1107,7 @@ int run_job(b200c_job* j, int until) {
   CU(j->run_bounds.reserve(16 * (size_t)(K + 1)));
   CU(j->run_first_d.reserve(4 * (size_t)(K + 2)));
   if (int rc = upload_small(j, j->run_first_d.p, run_first.data(), 4 * (size_t)(K + 1))) return rc;
-  launch_run_bounds(decc, j->run_start.as<uint64_t>(), j->run_first_d.as<uint32_t>(), K, j->run_bounds.as<uint64_t>(), err, st);
-  j->launches++;
+  launch_run_bounds(decc, j->run_start.as<uint64_t>(), j->run_first_d.as<uint32_t>(), K, j->run_bounds.as<uint64_t>(), err, st, &j->launches);
   RunBounds runs{j->run_bounds.as<uint64_t>(), j->run_bounds.as<uint64_t>() + K};
   // ---------------- sub-compaction key range: clip every run, the merge and everything behind it only see [start, end)
   const bool clipped = P.has_range_start || P.has_range_end;
@@ -1136,9 +1117,8 @@ int run_job(b200c_job* j, int until) {
     CU(j->clip_d.reserve(16 * (size_t)(K + 1)));
     j->kt_begin("merge.clip");
     launch_clip_runs(decc, runs, K, j->range_lo, P.has_range_start, j->range_hi, P.has_range_end,
-                     j->clip_d.as<uint64_t>(), reinterpret_cast<unsigned long long*>(small + kSlotClip), st);
+                     j->clip_d.as<uint64_t>(), reinterpret_cast<unsigned long long*>(small + kSlotClip), st, &j->launches);
     j->kt_end();
-    j->launches++;
     uint64_t hc[kSmallSlots];
     if (int rc = checked_sync(j, hc)) return rc;  // sync: the merge grid depends on the number of entries in range
     N_in = hc[kSlotClip];
@@ -1188,7 +1168,7 @@ int run_merge_encode(b200c_job* j, int until, KeyCols decc, RunBounds runs, uint
   W.totals = small + kSlotTotals;
   if (N) {
     j->kt_begin("merge.partition");
-    launch_merge_partition(decc, runs, (uint32_t)k, N, mtiles, j->splits.as<uint64_t>(), err, j->sms, st);
+    launch_merge_partition(decc, runs, (uint32_t)k, N, mtiles, j->splits.as<uint64_t>(), err, j->sms, st, &j->launches);
     j->kt_end();
     // the merge kernel also writes what the encoder needs per entry (encoded size, shared-prefix length) and per tile (statistics)
     const MergeSizes msz{W.esz, W.eshared, W.tstat, W.min_s1};
@@ -1196,12 +1176,12 @@ int run_merge_encode(b200c_job* j, int until, KeyCols decc, RunBounds runs, uint
     W.nstat = mtiles;
     j->kt_begin("merge.tiles");
     launch_merge_tiles(decc, runs, mp, N, mtiles, j->splits.as<uint64_t>(),
-                       j->tile_state.as<unsigned long long>(), reinterpret_cast<uint32_t*>(small + kSlotTicket), j->mrg.mut(), counters, msz, err, st);
+                       j->tile_state.as<unsigned long long>(), reinterpret_cast<uint32_t*>(small + kSlotTicket), j->mrg.mut(), counters, msz, err, st,
+                       &j->launches);
     j->kt_end();
     j->kt_begin("merge.sizes_fix");
-    launch_merge_sizes_fix(j->mrg.cols(0), j->tile_state.as<unsigned long long>(), mtiles, msz, st);
+    launch_merge_sizes_fix(j->mrg.cols(0), j->tile_state.as<unsigned long long>(), mtiles, msz, st, &j->launches);
     j->kt_end();
-    j->launches += 3;
   }
   CU(cudaEventRecord(j->ev[2], st));
   uint64_t h[kSmallSlots];
@@ -1416,13 +1396,10 @@ int b200c_job_add_input(b200c_job* j, int level, uint64_t file_number, const voi
     // executor plugin) gets the PCIe transfer of file i overlapped with the read of file i + 1.  Failures here are not errors: the
     // run copies the file itself when no eager copy is pending.
     if (cudaSetDevice(j->p.device) == cudaSuccess && (j->st_up || cudaStreamCreateWithFlags(&j->st_up, cudaStreamNonBlocking) == cudaSuccess) &&
-        in.staged.reserve(len + 64) == cudaSuccess && cudaEventCreateWithFlags(&in.up_ev, cudaEventDisableTiming) == cudaSuccess &&
-        cudaMemcpyAsync(in.staged.p, data, len, cudaMemcpyHostToDevice, j->st_up) == cudaSuccess &&
-        cudaEventRecord(in.up_ev, j->st_up) == cudaSuccess) {
-      in.uploaded = true;
-    } else {
+        stage_input(in, j->st_up, false) == B200C_OK)
+      in.copy.fresh = true;
+    else
       cudaGetLastError();
-    }
   }
   return B200C_OK;
 }
@@ -1437,18 +1414,16 @@ int b200c_job_plan_ranges(b200c_job* j, uint32_t max_ranges, uint64_t min_range_
   *n_boundaries = 0;
   if (max_ranges <= 1 || j->inputs.empty()) return B200C_OK;
   if (b200c_device_count() <= 0) return fail(B200C_ERR_NO_DEVICE, "no CUDA device");
-  CU(cudaSetDevice(j->p.device));
+  if (int rc = job_bind(j)) return rc;
   std::vector<Anchor> anchors;
   uint64_t total = 0;
-  std::vector<uint8_t> idx;
+  IndexBlock idx;
   for (Input& in : j->inputs) {
-    if (int rc = fetch_tail(j, in)) return rc;
+    if (int rc = open_input(j, in)) return rc;
     total += in.tail.data_size ? in.tail.data_size : in.len;
     if (in.tail.num_data_blocks < 2) continue;
-    const uint8_t* blk;
-    uint64_t blk_len;
-    if (int rc = host_index_block(in, &idx, &blk, &blk_len)) return rc;
-    const std::string e = index_anchors(blk, blk_len, in.tail, 128, &anchors);
+    if (int rc = input_index_block(j, in, &idx)) return rc;
+    const std::string e = index_anchors(idx.p, idx.len, in.tail, 128, &anchors);
     if (!e.empty()) return fail(B200C_ERR_CORRUPTION, e);
   }
   const std::vector<Anchor> bnd = plan_boundaries(std::move(anchors), total, max_ranges, min_range_bytes);
@@ -1467,16 +1442,11 @@ int b200c_job_create_sub(b200c_job* parent, const b200c_params* p, b200c_job** o
   if (p->device != parent->p.device) return fail(B200C_ERR_INVALID_ARGUMENT, "a sub-job runs on its parent's device");
   if (parent->inputs.empty()) return fail(B200C_ERR_STATE, "parent job has no inputs");
   CU(cudaSetDevice(parent->p.device));
-  // the device copies of the parent's host inputs: made once, here at the latest
+  // the device copies of the parent's host inputs, complete before a sub-job reads them (range-pipelined: it waits for its event)
   for (Input& in : parent->inputs) {
-    if (in.mem_kind != B200C_MEM_HOST || !parent->range_events.empty()) continue;  // (range-pipelined: the sub-job waits for its event)
-    if (in.uploaded) {
-      CU(cudaEventSynchronize(in.up_ev));
-    } else if (!in.shared_copy) {
-      CU(in.staged.reserve(in.len + 64));
-      CU(cudaMemcpy(in.staged.p, in.data, in.len, cudaMemcpyHostToDevice));
-    }
-    in.shared_copy = true;  // (a later run of the parent itself would still copy again: see run_job)
+    if (in.mem_kind != B200C_MEM_HOST || !parent->range_events.empty()) continue;
+    if (int rc = stage_input(in, nullptr, true)) return rc;
+    CU(cudaEventSynchronize(in.copy.done));
   }
   b200c_job* j = nullptr;
   if (int rc = b200c_job_create(p, &j)) return rc;
@@ -1487,7 +1457,7 @@ int b200c_job_create_sub(b200c_job* parent, const b200c_params* p, b200c_job** o
     s.file_number = in.file_number;
     s.len = in.len;
     s.mem_kind = B200C_MEM_DEVICE;
-    s.data = in.mem_kind == B200C_MEM_HOST ? in.staged.as<uint8_t>() : in.data;
+    s.data = in.mem_kind == B200C_MEM_HOST ? in.copy.buf.as<uint8_t>() : in.data;
   }
   if (!parent->range_events.empty()) {
     // the range that ends at boundary r needs the uploads up to event r; an open end (or a bound that is not one of the boundaries)
@@ -1512,7 +1482,7 @@ int b200c_job_upload_by_ranges(b200c_job* j, const uint8_t* keys, const uint32_t
   if (j->inputs.empty()) return fail(B200C_ERR_STATE, "job has no inputs");
   if (!j->range_events.empty()) return fail(B200C_ERR_STATE, "the inputs of this job are already uploaded by ranges");
   if (b200c_device_count() <= 0) return fail(B200C_ERR_NO_DEVICE, "no CUDA device");
-  CU(cudaSetDevice(j->p.device));
+  if (int rc = job_bind(j)) return rc;
   if (!j->st_up) CU(cudaStreamCreateWithFlags(&j->st_up, cudaStreamNonBlocking));
   std::vector<Anchor> bounds(nb);
   for (uint32_t r = 0; r < nb; r++) {
@@ -1525,39 +1495,32 @@ int b200c_job_upload_by_ranges(b200c_job* j, const uint8_t* keys, const uint32_t
   const size_t k = j->inputs.size();
   std::vector<std::vector<uint64_t>> cuts(k, std::vector<uint64_t>(nb, 0));  // end of chunk r inside file f's data region
   std::vector<uint64_t> data_end(k, 0);
-  std::vector<uint8_t> idx;
+  IndexBlock idx;
   for (size_t f = 0; f < k; f++) {
     Input& in = j->inputs[f];
-    if (in.mem_kind != B200C_MEM_HOST || in.uploaded)
+    if (in.mem_kind != B200C_MEM_HOST || in.copy.fresh)
       return fail(B200C_ERR_STATE, "upload by ranges needs host inputs added with B200C_MEM_HOST_DEFERRED");
-    if (int rc = fetch_tail(j, in)) return rc;
-    const uint8_t* blk;
-    uint64_t blk_len;
-    if (int rc = host_index_block(in, &idx, &blk, &blk_len)) return rc;
-    const std::string e = index_range_cuts(blk, blk_len, in.tail, in.len, bounds.data(), nb, cuts[f].data(), &data_end[f]);
+    if (int rc = open_input(j, in)) return rc;
+    if (int rc = input_index_block(j, in, &idx)) return rc;
+    const std::string e = index_range_cuts(idx.p, idx.len, in.tail, in.len, bounds.data(), nb, cuts[f].data(), &data_end[f]);
     if (!e.empty()) return fail(B200C_ERR_CORRUPTION, e);
-    CU(in.staged.reserve(in.len + 64));
+    CU(in.copy.buf.reserve(in.len + 64));  // every buffer before the first copy: a refusal leaves no copy in flight
   }
   // 1. what every range needs of every file: everything behind the data blocks (filter, index, properties, metaindex, footer)
-  for (size_t f = 0; f < k; f++) {
-    Input& in = j->inputs[f];
-    if (in.len > data_end[f])
-      CU(cudaMemcpyAsync(in.staged.as<uint8_t>() + data_end[f], in.data + data_end[f], in.len - data_end[f], cudaMemcpyHostToDevice, j->st_up));
-  }
+  for (size_t f = 0; f < k; f++)
+    if (int rc = stage_input(j->inputs[f], j->st_up, false, data_end[f])) return rc;
   // 2. the data blocks, range after range
   j->range_events.resize((size_t)nb + 1, nullptr);
   for (uint32_t r = 0; r <= nb; r++) {
     for (size_t f = 0; f < k; f++) {
-      Input& in = j->inputs[f];
       const uint64_t lo = r == 0 ? 0 : cuts[f][r - 1], hi = r == nb ? data_end[f] : cuts[f][r];
-      if (hi > lo) CU(cudaMemcpyAsync(in.staged.as<uint8_t>() + lo, in.data + lo, hi - lo, cudaMemcpyHostToDevice, j->st_up));
+      if (int rc = stage_input(j->inputs[f], j->st_up, false, lo, hi)) return rc;
     }
     CU(cudaEventCreateWithFlags(&j->range_events[r], cudaEventDisableTiming));
     CU(cudaEventRecord(j->range_events[r], j->st_up));
   }
   j->range_bounds.clear();
   for (uint32_t r = 0; r < nb; r++) j->range_bounds.emplace_back(reinterpret_cast<const char*>(bounds[r].key), bounds[r].klen);
-  for (Input& in : j->inputs) in.shared_copy = true;
   return B200C_OK;
 }
 
@@ -1635,7 +1598,7 @@ void b200c_job_destroy(b200c_job* j) {
   for (cudaEvent_t e : j->range_events)
     if (e) cudaEventDestroy(e);
   for (auto& in : j->inputs)
-    if (in.up_ev) cudaEventDestroy(in.up_ev);
+    if (in.copy.done) cudaEventDestroy(in.copy.done);
   if (j->st_up) cudaStreamDestroy(j->st_up);
   for (auto& kt : j->ktimes) {
     cudaEventDestroy(kt.a);

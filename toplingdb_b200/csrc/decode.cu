@@ -780,16 +780,23 @@ __global__ void meta_vlen_kernel(const uint32_t* __restrict__ meta, uint64_t n, 
 //                             (varint32 prefix, compress_format_version 2) -> its slot size in the arena
 //   (exclusive scan)          arena offsets
 //   verify_compressed_kernel  warp per compressed block: the block checksum covers the STORED bytes (block_fetcher.cc:32-40)
-//   inflate_blocks_kernel     thread per compressed block: raw deflate (inflate_rules.h) into its arena slot + an uncompressed trailer,
-//                             then the block's handle is redirected to the arena.  32 blocks per warp run the same decoder loops.
-constexpr uint8_t kZlibCompressionType = 2;  // CompressionType::kZlibCompression (include/rocksdb/compression_type.h)
+//   inflate_blocks_kernel     warp per compressed block: lane 0 inflates it (inflate_rules.h) into a shared-memory window, the warp
+//                             copies it with an uncompressed trailer to its arena slot, then the block's handle is redirected there.
+// A data block may announce 4 <= u < 2^31 bytes: 4 is the smallest block the block decoder reads (handle_in_file), the rule a stored
+// block meets too; below 2^31 a slot size and blk_size fit 32 bits.  An index block has its own bounds (api.cu input_index_block).
 __device__ __forceinline__ bool compressed_prefix(const uint8_t* p, uint32_t size, uint32_t* usize, uint32_t* hdr) {
   uint64_t u = 0;
-  const int c = get_varint(p, p + (size < 5 ? size : 5), &u);
+  const int c = inf_size_prefix(p, size, &u);
   if (c == 0 || u > 0x7fffffffull) return false;
   *usize = (uint32_t)u;
   *hdr = (uint32_t)c;
   return true;
+}
+// the bytes a compressed block takes in the arena: the inflated block and its trailer, to 16 bytes; 0: its size prefix is refused
+__device__ __forceinline__ uint32_t arena_slot(const uint8_t* p, uint32_t size, uint32_t& u, uint32_t& h) {
+  uint32_t s = 0;
+  if (compressed_prefix(p, size, &u, &h) && u >= 4) s = (u + 5 + 15) & ~15u;
+  return s;
 }
 __global__ void block_usize_kernel(const FileDesc* __restrict__ files, const uint64_t* __restrict__ blk_off, const uint32_t* __restrict__ blk_size,
                                    uint32_t nblk, uint32_t* __restrict__ slot, uint32_t* __restrict__ err) {
@@ -803,8 +810,8 @@ __global__ void block_usize_kernel(const FileDesc* __restrict__ files, const uin
     const uint8_t ctype = p[size];
     if (ctype == kZlibCompressionType) {
       uint32_t u, h;
-      if (compressed_prefix(p, size, &u, &h) && u >= 4) s = (u + 5 + 15) & ~15u;
-      else atomicOr(err, kErrCorruptBlock);
+      s = arena_slot(p, size, u, h);
+      if (s == 0) atomicOr(err, kErrCorruptBlock);
     } else if (ctype != 0) {
       atomicOr(err, kErrCompressed);  // a codec the device does not decode
     }
@@ -853,7 +860,7 @@ inflate_blocks_kernel(const FileDesc* __restrict__ files, uint64_t* __restrict__
     const uint8_t* p = files[bo >> kBlkFileShift].base + (bo & kBlkOffMask);
     const uint32_t size = blk_size[b];
     uint32_t u = 0, h = 0;
-    compressed_prefix(p, size, &u, &h);
+    const uint32_t slot_bytes = arena_slot(p, size, u, h);
     uint8_t* dst = arena + slot_off[b];
     const bool windowed = u <= kInflateWindow;
     long n = 0;
@@ -868,13 +875,13 @@ inflate_blocks_kernel(const FileDesc* __restrict__ files, uint64_t* __restrict__
       continue;
     }
     __syncwarp();
-    if (windowed) {  // slots are 16-byte aligned and hold u + 5 bytes rounded up to 16
+    if (windowed) {  // slots are 16-byte aligned
       if (lane == 0) {
         ws.out[u] = 0;  // trailer of an uncompressed block; the checksum bytes are never read (cksum = 0 for arena blocks)
         ws.out[u + 1] = ws.out[u + 2] = ws.out[u + 3] = ws.out[u + 4] = 0;
       }
       __syncwarp();
-      const uint32_t nvec = (u + 5 + 15) >> 4;
+      const uint32_t nvec = slot_bytes >> 4;
       const uint4* src4 = reinterpret_cast<const uint4*>(ws.out);
       uint4* dst4 = reinterpret_cast<uint4*>(dst);
       for (uint32_t i = lane; i < nvec; i += 32) dst4[i] = src4[i];
@@ -890,11 +897,13 @@ inflate_blocks_kernel(const FileDesc* __restrict__ files, uint64_t* __restrict__
   }
 }
 void launch_block_usize(const FileDesc* files_dev, const uint64_t* blk_off, const uint32_t* blk_size, uint32_t nblk, uint32_t* slot, uint32_t* err,
-                        cudaStream_t st) {
-  if (nblk) block_usize_kernel<<<(nblk + 255) / 256, 256, 0, st>>>(files_dev, blk_off, blk_size, nblk, slot, err);
+                        cudaStream_t st, uint64_t* launches) {
+  if (nblk == 0) return;
+  block_usize_kernel<<<(nblk + 255) / 256, 256, 0, st>>>(files_dev, blk_off, blk_size, nblk, slot, err);
+  *launches += 1;
 }
 void launch_inflate_blocks(const FileDesc* files_dev, uint64_t* blk_off, uint32_t* blk_size, const uint32_t* slot, const uint64_t* slot_off,
-                           uint32_t nblk, uint8_t* arena, uint32_t verify, uint32_t* err, int sms, cudaStream_t st) {
+                           uint32_t nblk, uint8_t* arena, uint32_t verify, uint32_t* err, int sms, cudaStream_t st, uint64_t* launches) {
   if (nblk == 0) return;
   if (verify) {
     unsigned g = (nblk + 7) / 8;
@@ -911,18 +920,20 @@ void launch_inflate_blocks(const FileDesc* files_dev, uint64_t* blk_off, uint32_
   unsigned grid = (nblk + kInflateWarps - 1) / kInflateWarps;
   if (grid > (unsigned)sms * 3u) grid = (unsigned)sms * 3u;  // three CTAs (24 warps) per SM, each warp walks its share of the blocks
   inflate_blocks_kernel<<<grid, kInflateWarps * 32, smem, st>>>(files_dev, blk_off, blk_size, slot, slot_off, nblk, arena, err);
+  *launches += verify ? 2 : 1;
 }
 
 // ---------------------------------------------------------------------------------------------- host launchers
-void launch_index_decode(const FileDesc* files_dev, int nfiles, uint32_t max_blocks_per_file, uint64_t* blk_off,
-                         uint32_t* blk_size, BoundKey start, uint32_t has_start, BoundKey end, uint32_t has_end, uint32_t* err, cudaStream_t st) {
+void launch_index_decode(const FileDesc* files_dev, int nfiles, uint32_t max_blocks_per_file, uint64_t* blk_off, uint32_t* blk_size,
+                         BoundKey start, uint32_t has_start, BoundKey end, uint32_t has_end, uint32_t* err, cudaStream_t st, uint64_t* launches) {
   dim3 grid((max_blocks_per_file + 255) / 256 ? (max_blocks_per_file + 255) / 256 : 1, nfiles);
   if (grid.x > 1024) grid.x = 1024;
   index_decode_kernel<<<grid, 256, 0, st>>>(files_dev, nfiles, blk_off, blk_size, start, has_start, end, has_end, err);
+  *launches += 1;
 }
 void launch_block_decode_fused(const FileDesc* files_dev, int nfiles, const uint64_t* blk_off, const uint32_t* blk_size, uint32_t nblk,
                                uint32_t verify, uint64_t n_total, KeyColsMut out, unsigned long long* blk_state, uint32_t* ticket,
-                               uint64_t* run_start, uint64_t* total_out, uint32_t* err, int sms, cudaStream_t st, const uint8_t* arena) {
+                               uint64_t* run_start, uint64_t* total_out, uint32_t* err, int sms, cudaStream_t st, uint64_t* launches, const uint8_t* arena) {
   const int smem = kDecWarps * (int)sizeof(DecWarpSmem);
   static_assert(kDecCtasPerSm * (kDecWarps * sizeof(DecWarpSmem) + 4096) <= 227 * 1024, "four decode CTAs must fit one SM");
   static PerDeviceFlag attr;
@@ -936,6 +947,7 @@ void launch_block_decode_fused(const FileDesc* files_dev, int nfiles, const uint
   const unsigned grid = want < cap ? (want ? want : 1) : cap;
   const DecodeJob job{files_dev, nfiles, nblk, n_total, out, blk_state, run_start, total_out, err};
   block_decode_fused_kernel<<<grid, kDecWarps * 32, smem, st>>>(job, blk_off, blk_size, verify, ticket, arena);
+  *launches += 1;
 }
 void launch_gather_values(KeyCols in, const uint64_t* dst_off, uint8_t* dst, cudaStream_t st) {
   if (in.n == 0) return;
@@ -972,10 +984,11 @@ __global__ void compare_columns_kernel(KeyCols a, KeyCols b, uint64_t n, uint32_
 }
 __global__ void flip_byte_kernel(uint8_t* p) { *p ^= 0x40; }
 void launch_flip_byte(uint8_t* p, cudaStream_t st) { flip_byte_kernel<<<1, 1, 0, st>>>(p); }
-void launch_compare_columns(KeyCols written, KeyCols reread, uint64_t n, uint32_t* err, int sms, cudaStream_t st) {
+void launch_compare_columns(KeyCols written, KeyCols reread, uint64_t n, uint32_t* err, int sms, cudaStream_t st, uint64_t* launches) {
   if (n == 0) return;
   const uint64_t blocks = (n + 255) / 256;
   compare_columns_kernel<<<(unsigned)(blocks < (unsigned)sms * 16 ? blocks : (unsigned)sms * 16), 256, 0, st>>>(written, reread, n, err);
+  *launches += 1;
 }
 
 }  // namespace b200c

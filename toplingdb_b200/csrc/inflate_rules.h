@@ -3,10 +3,10 @@
 // The reference stores a kZlibCompression block as  varint32 uncompressed_size ‖ raw deflate stream  (Zlib_Compress,
 // util/compression.h:746-826: compress_format_version 2, window_bits -14 = no zlib header / Adler-32) and reads it back with
 // Zlib_Uncompress (:834-924) from UncompressBlockData (table/format.cc:511).  On the device every compressed block is inflated by
-// ONE THREAD (decode.cu inflate_blocks_kernel): the 32 lanes of a warp run the same loops over 32 different blocks, so the decoder
-// is written as plain sequential code without tables larger than a thread's local memory: canonical Huffman decoding by code
-// length (count[] / symbol[] per code, one bit per step).  tests/test_inflate_rules_host.py compiles this header for the host and
-// checks it against zlib on reference-written blocks and on random streams of all three block types.
+// ONE WARP (decode.cu inflate_blocks_kernel): lane 0 runs this sequential decoder with its tables and output window in shared memory;
+// the host runs it on compressed index blocks (api.cu).  Canonical Huffman decoding: a first-level table, then by code length
+// (count[] / symbol[] per code, one bit per step).  tests/test_inflate_rules_host.py compiles this header for the host and checks it
+// against zlib on reference-written blocks and on random streams of all three block types.
 #pragma once
 #include <stdint.h>
 
@@ -51,9 +51,9 @@ struct InfHuff {  // canonical code: count[len] codes of each length, symbols or
   uint16_t* count;   // [kInfMaxBits + 1]
   uint16_t* symbol;
 };
-// The decoder's tables.  On the device they live in SHARED memory, one slice per thread (as thread-local arrays they go to local
+// The decoder's tables.  On the device they live in SHARED memory, one slice per warp (as thread-local arrays they go to local
 // memory, and with tens of thousands of blocks in flight every count[] / symbol[] probe of the bit-by-bit decode was an L2 round
-// trip).  257 words: consecutive threads' slices start in different banks.
+// trip).
 constexpr int kInfLBits = 9, kInfDBits = 6;  // first-level lookup: codes of up to this many bits decode with one table probe
 struct InfWork {
   uint16_t lcount[kInfMaxBits + 1], dcount[kInfMaxBits + 1];
@@ -250,6 +250,26 @@ B200C_INF_HD inline long inflate_raw(const uint8_t* src, uint32_t n, uint8_t* ds
     if (last) break;
   }
   return (long)out;
+}
+
+constexpr uint8_t kZlibCompressionType = 2;  // block trailer type byte of kZlibCompression (include/rocksdb/compression_type.h)
+// The varint32 prefix of a compressed block p[0, size): its length in bytes, 0 when it does not end within the block's first five
+// bytes; the announced uncompressed size in *u.  Each caller bounds *u by what it accepts.
+B200C_INF_HD inline int inf_size_prefix(const uint8_t* p, uint32_t size, uint64_t* u) {
+  const uint8_t* end = p + (size < 5 ? size : 5);
+  uint64_t r = 0;
+  int n = 0;
+#pragma unroll 1
+  for (int s = 0; s <= 28; s += 7) {
+    if (p + n >= end) return 0;
+    const uint8_t c = p[n++];
+    r |= (uint64_t)(c & 127) << s;
+    if (c < 128) {
+      *u = r;
+      return n;
+    }
+  }
+  return 0;
 }
 
 }  // namespace b200c

@@ -44,23 +44,23 @@ struct BoundKey {              // a user key in column form (grandparent boundar
 // ---- decode.cu
 // blk_size[b] == 0 marks a data block that a sub-compaction's key range [start, end) cannot touch (range_rules.h): the block decoder
 // publishes an empty block for it without reading the image
-void launch_index_decode(const FileDesc* files_dev, int nfiles, uint32_t max_blocks_per_file, uint64_t* blk_off,
-                         uint32_t* blk_size, BoundKey start, uint32_t has_start, BoundKey end, uint32_t has_end, uint32_t* err, cudaStream_t st);
+void launch_index_decode(const FileDesc* files_dev, int nfiles, uint32_t max_blocks_per_file, uint64_t* blk_off, uint32_t* blk_size,
+                         BoundKey start, uint32_t has_start, BoundKey end, uint32_t has_end, uint32_t* err, cudaStream_t st, uint64_t* launches);
 void launch_block_decode_fused(const FileDesc* files_dev, int nfiles, const uint64_t* blk_off, const uint32_t* blk_size, uint32_t nblk,
                                uint32_t verify, uint64_t n_total, KeyColsMut out, unsigned long long* blk_state, uint32_t* ticket,
-                               uint64_t* run_start, uint64_t* total_out, uint32_t* err, int sms, cudaStream_t st,
+                               uint64_t* run_start, uint64_t* total_out, uint32_t* err, int sms, cudaStream_t st, uint64_t* launches,
                                const uint8_t* arena = nullptr);
 // Inputs with kZlibCompression data blocks (UncompressBlockData, table/format.cc:511): slot[b] = bytes block b needs in the arena of
 // inflated blocks (0: stored uncompressed / outside the key range); after an exclusive scan of the slots, launch_inflate_blocks verifies
 // the stored bytes' checksums, inflates every compressed block into its slot and redirects its handle (blk_off / blk_size) there.
 void launch_block_usize(const FileDesc* files_dev, const uint64_t* blk_off, const uint32_t* blk_size, uint32_t nblk, uint32_t* slot, uint32_t* err,
-                        cudaStream_t st);
+                        cudaStream_t st, uint64_t* launches);
 void launch_inflate_blocks(const FileDesc* files_dev, uint64_t* blk_off, uint32_t* blk_size, const uint32_t* slot, const uint64_t* slot_off,
-                           uint32_t nblk, uint8_t* arena, uint32_t verify, uint32_t* err, int sms, cudaStream_t st);
+                           uint32_t nblk, uint8_t* arena, uint32_t verify, uint32_t* err, int sms, cudaStream_t st, uint64_t* launches);
 // paranoid_file_checks: entry i of `written` (what the encoder consumed) and of `reread` (the output images decoded again) must be
 // the same key, the same trailer and the same value bytes; a difference sets kErrParanoid
 void launch_flip_byte(uint8_t* p, cudaStream_t st);  // test hook of paranoid_file_checks
-void launch_compare_columns(KeyCols written, KeyCols reread, uint64_t n, uint32_t* err, int sms, cudaStream_t st);
+void launch_compare_columns(KeyCols written, KeyCols reread, uint64_t n, uint32_t* err, int sms, cudaStream_t st, uint64_t* launches);
 void launch_gather_values(KeyCols in, const uint64_t* dst_off, uint8_t* dst, cudaStream_t st);
 void launch_meta_vlen(const uint32_t* meta, uint64_t n, uint32_t* vlen, cudaStream_t st);
 // host records (internal key + value, back to back) -> key columns with value references into the device arena
@@ -123,18 +123,18 @@ struct RunBounds {
 // start <= user key < end.  clip[r] / clip[nruns + r] = first / one-past-last entry of run r in range; totals[0] += entries in
 // range, totals[1] += their value bytes.
 void launch_clip_runs(KeyCols in, RunBounds runs, uint32_t nruns, BoundKey start, uint32_t has_start, BoundKey end,
-                      uint32_t has_end, uint64_t* clip, unsigned long long* totals, cudaStream_t st);
+                      uint32_t has_end, uint64_t* clip, unsigned long long* totals, cudaStream_t st, uint64_t* launches);
 // Sorted runs from decoded files: run r = the files [run_first[r], run_first[r + 1]), decoded back to back; bounds = begin[nruns] |
 // end[nruns].  Checks that consecutive files of one run are in order (a level's files are disjoint and sorted): kErrKeyOrder.
 void launch_run_bounds(KeyCols in, const uint64_t* file_start, const uint32_t* run_first, uint32_t nruns, uint64_t* bounds, uint32_t* err,
-                       cudaStream_t st);
+                       cudaStream_t st, uint64_t* launches);
 void launch_merge_partition(KeyCols in, RunBounds runs, uint32_t nruns, uint64_t n_total, uint64_t ntiles,
-                            uint64_t* splits, uint32_t* err, int sms, cudaStream_t st);
+                            uint64_t* splits, uint32_t* err, int sms, cudaStream_t st, uint64_t* launches);
 void launch_merge_tiles(KeyCols in, RunBounds runs, MergeParams mp, uint64_t n_total, uint64_t ntiles,
                         const uint64_t* splits, unsigned long long* tile_state, uint32_t* ticket, KeyColsMut out,
-                        MergeCounters* counters, MergeSizes ms, uint32_t* err, cudaStream_t st);
+                        MergeCounters* counters, MergeSizes ms, uint32_t* err, cudaStream_t st, uint64_t* launches);
 // sizes of each tile's first output entry (needs the finished tile_state prefixes and merged columns)
-void launch_merge_sizes_fix(KeyCols merged, const unsigned long long* tile_state, uint64_t ntiles, MergeSizes ms, cudaStream_t st);
+void launch_merge_sizes_fix(KeyCols merged, const unsigned long long* tile_state, uint64_t ntiles, MergeSizes ms, cudaStream_t st, uint64_t* launches);
 
 // ---- encode.cu
 // Grandparent-aware output cutting (CompactionOutputs::ShouldStopBefore, compaction_outputs.cc:231-354).  The walk over the block

@@ -1138,8 +1138,10 @@ clip_runs_kernel(KeyCols in, RunBounds runs, uint32_t nruns, BoundKey start, uin
   if ((threadIdx.x & 31) == 0 && sum) atomicAdd(&totals[1], sum);
 }
 void launch_clip_runs(KeyCols in, RunBounds runs, uint32_t nruns, BoundKey start, uint32_t has_start, BoundKey end,
-                      uint32_t has_end, uint64_t* clip, unsigned long long* totals, cudaStream_t st) {
-  if (nruns) clip_runs_kernel<<<dim3(kClipSlices, nruns), 256, 0, st>>>(in, runs, nruns, start, has_start, end, has_end, clip, totals);
+                      uint32_t has_end, uint64_t* clip, unsigned long long* totals, cudaStream_t st, uint64_t* launches) {
+  if (nruns == 0) return;
+  clip_runs_kernel<<<dim3(kClipSlices, nruns), 256, 0, st>>>(in, runs, nruns, start, has_start, end, has_end, clip, totals);
+  *launches += 1;
 }
 // one thread per run: its column range, and the order of the files inside it
 __global__ void run_bounds_kernel(KeyCols in, const uint64_t* __restrict__ file_start, const uint32_t* __restrict__ run_first, uint32_t nruns,
@@ -1155,13 +1157,16 @@ __global__ void run_bounds_kernel(KeyCols in, const uint64_t* __restrict__ file_
   }
 }
 void launch_run_bounds(KeyCols in, const uint64_t* file_start, const uint32_t* run_first, uint32_t nruns, uint64_t* bounds, uint32_t* err,
-                       cudaStream_t st) {
-  if (nruns) run_bounds_kernel<<<(nruns + 63) / 64, 64, 0, st>>>(in, file_start, run_first, nruns, bounds, err);
+                       cudaStream_t st, uint64_t* launches) {
+  if (nruns == 0) return;
+  run_bounds_kernel<<<(nruns + 63) / 64, 64, 0, st>>>(in, file_start, run_first, nruns, bounds, err);
+  *launches += 1;
 }
 
 // ------------------------------------------------------------------------------------------------ launchers
 void launch_merge_partition(KeyCols in, RunBounds runs, uint32_t nruns, uint64_t n_total, uint64_t ntiles,
-                            uint64_t* splits, uint32_t* err, int sms, cudaStream_t st) {
+                            uint64_t* splits, uint32_t* err, int sms, cudaStream_t st, uint64_t* launches) {
+  *launches += 1;
   unsigned warps = (unsigned)(ntiles + 1);
   if (nruns <= kPartGroupedMaxRuns) {
     uint32_t kp2 = 2;  // at most 16 lanes per run
@@ -1183,7 +1188,7 @@ static_assert(sizeof(Key) * kMaxRuns <= sizeof(uint64_t) * kMT && 4 * kMaxRuns <
 static_assert(kMergeCtasPerSm * (sizeof(TileSmem) + 1024) <= 227 * 1024, "merge tile must fit three CTAs per SM");
 void launch_merge_tiles(KeyCols in, RunBounds runs, MergeParams mp, uint64_t n_total, uint64_t ntiles,
                         const uint64_t* splits, unsigned long long* tile_state, uint32_t* ticket, KeyColsMut out,
-                        MergeCounters* counters, MergeSizes ms, uint32_t* err, cudaStream_t st) {
+                        MergeCounters* counters, MergeSizes ms, uint32_t* err, cudaStream_t st, uint64_t* launches) {
   if (ntiles == 0) return;
   static PerDeviceFlag attr;
   const uint64_t dev_bit = attr.bit_of_current_device();
@@ -1196,9 +1201,12 @@ void launch_merge_tiles(KeyCols in, RunBounds runs, MergeParams mp, uint64_t n_t
                                                                                    out, counters, ms, err);
   merge_tiles_kernel<true><<<(unsigned)ntiles, kMThreads, sizeof(TileSmem), st>>>(in, runs, mp, n_total, ntiles, splits, tile_state, ticket,
                                                                                   out, counters, ms, err);
+  *launches += 1;  // the pair counts as one launch: the variant that does not apply leaves at once
 }
-void launch_merge_sizes_fix(KeyCols merged, const unsigned long long* tile_state, uint64_t ntiles, MergeSizes ms, cudaStream_t st) {
-  if (ntiles) merge_sizes_fix_kernel<<<(unsigned)((ntiles + 127) / 128), 128, 0, st>>>(merged, tile_state, ntiles, ms);
+void launch_merge_sizes_fix(KeyCols merged, const unsigned long long* tile_state, uint64_t ntiles, MergeSizes ms, cudaStream_t st, uint64_t* launches) {
+  if (ntiles == 0) return;
+  merge_sizes_fix_kernel<<<(unsigned)((ntiles + 127) / 128), 128, 0, st>>>(merged, tile_state, ntiles, ms);
+  *launches += 1;
 }
 
 }  // namespace b200c
